@@ -87,7 +87,8 @@ LEXP_API int lexp_set_volume_device(lexp_ctx* ctx, int mode, const float* vol_de
  *   LEXP_VOL_RIGHT_FROM_LEFT  (mode must be 1) `vol` is the LEFT volume as loaded (im0.acrt, not yet filled); the context's view-1
  *                             volume becomes fillOutOfView(convertVolumeL2R(fillOutOfView(vol, 0)), 1) (main.cpp:356-365), i.e.
  *                             volR[d][y][x] = volL[d][y][min(x + d, W-1)] -- no second volume on the host, no im1.acrt.
- * The host variant uploads in slabs of disparities (LEXP_UPLOAD_SLAB_MB, default 512): no second full-size device copy. */
+ * The host variant uploads in slabs of disparities (LEXP_UPLOAD_SLAB_MB, default 512, read by lexp_create): no second full-size
+ * device copy. */
 #define LEXP_VOL_PLAIN 0
 #define LEXP_VOL_FILL 1
 #define LEXP_VOL_RIGHT_FROM_LEFT 2

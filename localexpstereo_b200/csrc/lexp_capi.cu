@@ -106,7 +106,9 @@ struct lexp_ctx {
     float4* d_exi[2] = {nullptr, nullptr}; // NaiveStereoEnergy: ExI planes
     size_t gs_bytes = 0;
     size_t persist_bytes = 0;             // L2 set-aside for persisting accesses (0: unsupported)
+    bool persist_prefix = true;           // window = a prefix of the set-aside size, hit ratio 1 (LEXP_L2_PERSIST=2: the whole allocation)
     int persist_mode = -1;                // view whose window is currently installed on the stream
+    int upload_slab_mb = 512;             // staging of the host volume uploads (LEXP_UPLOAD_SLAB_MB)
     float* d_vol[2] = {nullptr, nullptr};   // blocked copy float[Hb][Wb][D][4][4] (owned)
     float* d_cur_cost[2] = {nullptr, nullptr};     // PatchMatch phase: currentCost_[mode]   float [H][W]
     float4* d_cur_label[2] = {nullptr, nullptr};   //                   currentLabeling_[mode] Plane[H][W]
@@ -143,7 +145,8 @@ struct lexp_ctx {
     bool chain_ok = false;       // the last operation this context put on its stream was a launch of lexp_fused_kernel: only then may the
                                  // next launch carry the programmatic-serialization attribute.  After a memcpy / memset (plane upload, counter
                                  // reset, state upload) the next launch is an ordinary one: a kernel launched with the attribute right after a
-                                 // copy was observed reading the copy's destination before the copy had landed
+                                 // copy was observed reading the copy's destination before the copy had landed.  Set by launch_fused_t, cleared
+                                 // by the stream helpers (h2d, d2h, memset0, launch_aux) and lexp_set_stream only
     size_t smem_cap = 0;         // upper bound on a work item's dynamic shared memory, 0: none (LEXP_SMEM_CAP)
     size_t smem_limit = 0;
     size_t window_max = 0;
@@ -196,13 +199,47 @@ struct lexp_ctx {
 #if LEXP_TRACE
     long long* d_trace = nullptr;
     size_t trace_cap = 0;
+    std::string trace_file;   // LEXP_TRACE_FILE (empty: stderr)
 #endif
 };
 
+// Entry of a call that works on the context's device state: holds c->mu until the call returns and makes the context's device current.
+#define LEXP_ENTER(c)                                 \
+    std::lock_guard<std::mutex> ctx_lock_((c)->mu);   \
+    LEXP_CUDA(cudaSetDevice((c)->p.device))
+
 namespace {
 
+// Everything put on the context's stream besides lexp_fused_kernel goes through these four helpers (the exception: the diagnosis
+// reads of report_trace).  Each ends the chain of fused launches that may carry the programmatic-serialization attribute (chain_ok).
+cudaError_t h2d(lexp_ctx* c, void* dst, const void* src, size_t bytes) {
+    c->chain_ok = false;
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, c->stream);
+}
+cudaError_t d2h(lexp_ctx* c, void* dst, const void* src, size_t bytes) {
+    c->chain_ok = false;
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, c->stream);
+}
+cudaError_t memset0(lexp_ctx* c, void* dst, size_t bytes) {
+    c->chain_ok = false;
+    return cudaMemsetAsync(dst, 0, bytes, c->stream);
+}
+template <class... KArgs, class... Args>
+cudaError_t launch_aux(lexp_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, Args... args) {
+    c->chain_ok = false;
+    LEXP_LAUNCH(kern, grid, block, 0, c->stream, args...);
+    c->launches++;
+    return cudaGetLastError();
+}
+
+int require_pm_state(const lexp_ctx* c, int mode) {
+    if (!c->d_cur_cost[mode] || !c->d_cur_label[mode] || !c->d_flags[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
+    return LEXP_OK;
+}
+
 #if LEXP_TRACE
-// diagnosis build: per-team averages of {total cycles, waiting for input, waiting for an output buffer} of one launch
+// diagnosis build: per-team averages of {total cycles, waiting for input, waiting for an output buffer} of one launch.  Its reads
+// synchronise the stream first and do not go through the stream helpers: they leave the chain of fused launches as it is.
 void report_trace(lexp_ctx* c, int nitems) {
     constexpr int NW = kThreads / 32;
     std::vector<long long> h((size_t)nitems * NW * 4);
@@ -210,8 +247,8 @@ void report_trace(lexp_ctx* c, int nitems) {
     if (cudaMemcpy(h.data(), c->d_trace, h.size() * sizeof(long long), cudaMemcpyDeviceToHost) != cudaSuccess) return;
     const char* names[5] = {"A", "H1", "H2", "C", "E"};
     const int first[6] = {0, kWarpsA, kWarpsA + 1, kWarpsA + kWarpsH, kWarpsA + kWarpsH + kWarpsC, NW};
-    const char* path = getenv("LEXP_TRACE_FILE");
-    FILE* f = path ? fopen(path, "a") : stderr;
+    const bool to_file = !c->trace_file.empty();
+    FILE* f = to_file ? fopen(c->trace_file.c_str(), "a") : stderr;
     if (!f) return;
     double chunks = 0;
     for (int i = 0; i < nitems; i++) chunks += (double)(h[(size_t)i * NW * 4 + 3] & 0xffffffffLL);
@@ -228,7 +265,7 @@ void report_trace(lexp_ctx* c, int nitems) {
                 (tot - win - wout) / n, wld / n);
     }
     fprintf(f, "\n");
-    if (path) fclose(f);
+    if (to_file) fclose(f);
 }
 #endif
 
@@ -380,8 +417,7 @@ int run_plan(lexp_ctx* c, lexp_plan* pl, int mode, const Plane4* d_planes, float
         av.accessPolicyWindow.base_ptr = c->d_gs[mode];
         // default: pin a prefix [statA | statC | guide | ..] of exactly the set-aside size with hit ratio 1 (LEXP_L2_PERSIST=2:
         // the whole allocation with a fractional hit ratio instead)
-        const bool prefix = env_int("LEXP_L2_PERSIST", 1) != 2;
-        av.accessPolicyWindow.num_bytes = prefix ? std::min(c->gs_bytes, c->persist_bytes) : std::min(c->gs_bytes, c->window_max);
+        av.accessPolicyWindow.num_bytes = c->persist_prefix ? std::min(c->gs_bytes, c->persist_bytes) : std::min(c->gs_bytes, c->window_max);
         av.accessPolicyWindow.hitRatio = (float)std::min(1.0, (double)c->persist_bytes / (double)av.accessPolicyWindow.num_bytes);
         av.accessPolicyWindow.hitProp = cudaAccessPropertyPersisting;
         av.accessPolicyWindow.missProp = cudaAccessPropertyNormal;
@@ -436,12 +472,18 @@ int run_plan(lexp_ctx* c, lexp_plan* pl, int mode, const Plane4* d_planes, float
 // blocked copy, applying the volume-preparation transform of lexp_relayout_volume on the way.  Asynchronous; d_flag accumulates.
 int ingest_slab(lexp_ctx* c, int mode, const float* d_src, int d_lo, int nd, int transform, int* d_flag) {
     const int D = c->p.ndisp, H = c->p.height, W = c->p.width, Wb = (W + 3) / 4, Hb = (H + 3) / 4;
-    LEXP_LAUNCH(lexp_scan_nonfinite, c->num_sms * 8, 256, 0, c->stream, d_src, (size_t)nd * H * W, d_flag);
+    LEXP_CUDA(launch_aux(c, lexp_scan_nonfinite, c->num_sms * 8, 256, d_src, (size_t)nd * H * W, d_flag));
     dim3 grd((W + 31) / 32, Hb, (nd + 7) / 8);
-    LEXP_LAUNCH(lexp_relayout_volume, grd, 256, 0, c->stream, d_src, c->d_vol[mode], D, H, W, Wb, d_lo, nd, transform);
-    c->launches += 2;
-    LEXP_CUDA(cudaGetLastError());
+    LEXP_CUDA(launch_aux(c, lexp_relayout_volume, grd, 256, d_src, c->d_vol[mode], D, H, W, Wb, d_lo, nd, transform));
     return LEXP_OK;
+}
+
+// disparities per slab of a host volume upload: LEXP_UPLOAD_SLAB_MB of staging, at least 8, rounded up to a multiple of 8, at most D
+int upload_slab(const lexp_ctx* c) {
+    const int D = c->p.ndisp;
+    const size_t plane = (size_t)c->p.height * c->p.width;
+    const int slab = (int)std::max<size_t>(8, std::min<size_t>((size_t)D, ((size_t)c->upload_slab_mb << 20) / (plane * sizeof(float))));
+    return std::min(D, (slab + 7) / 8 * 8);
 }
 
 int check_transform(int mode, int transform) {
@@ -458,17 +500,71 @@ int alloc_volume(lexp_ctx* c, int mode, int** d_flag) {
     const int D = c->p.ndisp, H = c->p.height, W = c->p.width, Wb = (W + 3) / 4, Hb = (H + 3) / 4;
     if (!c->d_vol[mode]) LEXP_CUDA(cudaMalloc(&c->d_vol[mode], (size_t)Hb * Wb * D * 16 * sizeof(float)));
     LEXP_CUDA(cudaMalloc(d_flag, sizeof(int)));
-    LEXP_CUDA(cudaMemsetAsync(*d_flag, 0, sizeof(int), c->stream));
+    LEXP_CUDA(memset0(c, *d_flag, sizeof(int)));
     return LEXP_OK;
 }
 
 int finish_volume(lexp_ctx* c, int mode, int* d_flag) {
     int h = 1;
-    cudaError_t e = cudaMemcpyAsync(&h, d_flag, sizeof(int), cudaMemcpyDeviceToHost, c->stream);
+    cudaError_t e = d2h(c, &h, d_flag, sizeof(int));
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     cudaFree(d_flag);
     if (e != cudaSuccess) return fail(LEXP_ERR_CUDA, std::string("volume ingest: ") + cudaGetErrorString(e));
     c->vol_finite[mode] = (h == 0);
+    return LEXP_OK;
+}
+
+// The device address of a plan's planes: the caller's device array, or the plan's staging buffer after the host-to-device copy
+// (nullptr: the copy failed)
+const Plane4* stage_planes(lexp_ctx* c, lexp_plan* pl, const lexp_plane* planes, bool on_device) {
+    if (on_device) return reinterpret_cast<const Plane4*>(planes);
+    const cudaError_t e = h2d(c, pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4));
+    if (e != cudaSuccess) { fail(LEXP_ERR_CUDA, std::string("plane upload: ") + cudaGetErrorString(e)); return nullptr; }
+    return pl->d_planes;
+}
+
+// lexp_plan_eval_device (row pitch in floats) and lexp_plan_eval_device_tiles (compact tiles)
+int eval_device(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, int planes_on_device, float* d_out, long long pitch,
+                int compact, int with_check) {
+    LEXP_ENTER(c);
+    const Plane4* dp = stage_planes(c, pl, planes, planes_on_device);
+    if (!dp) return LEXP_ERR_CUDA;
+    return run_plan(c, pl, mode, dp, d_out, pitch, compact, with_check, nullptr, planes_on_device && c->overlap);
+}
+
+// The two host entry points.  d_direct: the device alias of the caller's output when mapped_alias accepted its whole range; the kernel
+// writes it (pitch / compact as for the device paths) and the stream is synchronised.  nullptr: the kernel writes the plan's compact buffer
+// and the caller copies it out.
+int eval_host(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, float* d_direct, long long pitch, int compact, int with_check) {
+    if (!d_direct) { int rc = ensure_compact(pl, (size_t)pl->sum_s); if (rc) return rc; }
+    const Plane4* dp = stage_planes(c, pl, planes, false);
+    if (!dp) return LEXP_ERR_CUDA;
+    if (!d_direct) return run_plan(c, pl, mode, dp, pl->d_compact, 0, 1, with_check);
+    { int rc = run_plan(c, pl, mode, dp, d_direct, pitch, compact, with_check); if (rc) return rc; }
+    LEXP_CUDA(cudaStreamSynchronize(c->stream));
+    return LEXP_OK;
+}
+
+// lexp_plan_eval_host through a plan that is destroyed right after; the evaluation's error message survives the destruction
+int eval_host_once(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, float* cost_image, ptrdiff_t step_bytes, int with_check) {
+    const int rc = lexp_plan_eval_host(c, pl, mode, planes, cost_image, step_bytes, with_check);
+    const std::string keep = g_err;
+    lexp_plan_destroy(pl);
+    g_err = keep;
+    return rc;
+}
+
+// Read-back of a derived image: `fill` launches into a temporary device buffer of `bytes`, whose bytes [at, at + out_bytes) are then
+// copied to `out`.  Synchronous.
+template <class Fill>
+int read_back(lexp_ctx* c, const char* what, size_t bytes, size_t at, void* out, size_t out_bytes, Fill fill) {
+    char* d = nullptr;
+    LEXP_CUDA(cudaMalloc(&d, bytes));
+    cudaError_t e = fill(d);
+    if (e == cudaSuccess) e = d2h(c, out, d + at, out_bytes);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+    cudaFree(d);
+    if (e != cudaSuccess) return fail(LEXP_ERR_CUDA, std::string(what) + ": " + cudaGetErrorString(e));
     return LEXP_OK;
 }
 
@@ -510,7 +606,13 @@ int lexp_create(const lexp_params* params, lexp_ctx** out_ctx) {
     c->gc_threads = std::min(1024, std::max(32, env_int("LEXP_GC_THREADS", 1024) / 32 * 32));
     c->gc_relabel_every = std::max(1, env_int("LEXP_GC_RELABEL_EVERY", 24));
     c->gc_big_nodes = std::max(0, env_int("LEXP_GC_BIG_NODES", 32768));
-    if (env_int("LEXP_L2_PERSIST", 1) && prop.persistingL2CacheMaxSize > 0) {
+    c->upload_slab_mb = env_int("LEXP_UPLOAD_SLAB_MB", 512);
+#if LEXP_TRACE
+    if (const char* path = getenv("LEXP_TRACE_FILE")) c->trace_file = path;
+#endif
+    const int l2_persist = env_int("LEXP_L2_PERSIST", 1);
+    c->persist_prefix = l2_persist != 2;
+    if (l2_persist && prop.persistingL2CacheMaxSize > 0) {
         const size_t want = (size_t)prop.persistingL2CacheMaxSize;
         if (cudaDeviceSetLimit(cudaLimitPersistingL2CacheSize, want) == cudaSuccess) {
             c->persist_bytes = want;
@@ -566,9 +668,7 @@ int lexp_destroy(lexp_ctx* c) {
 
 int lexp_set_image(lexp_ctx* c, int mode, const uint8_t* bgr, ptrdiff_t step) {
     if (!c || !bgr || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     const int H = c->p.height, W = c->p.width;
     const size_t HW = (size_t)H * W;
     c->coef_valid[mode] = false;
@@ -588,20 +688,18 @@ int lexp_set_image(lexp_ctx* c, int mode, const uint8_t* bgr, ptrdiff_t step) {
         c->d_statB[mode] = reinterpret_cast<float4*>(b + HWp * 24);
         c->gs_bytes = HWp * 40;
     }
-    LEXP_CUDA(cudaMemcpyAsync(c->d_guide[mode], tmp.data(), HW * sizeof(uchar4), cudaMemcpyHostToDevice, c->stream));
+    LEXP_CUDA(h2d(c, c->d_guide[mode], tmp.data(), HW * sizeof(uchar4)));
     int* d_rs = nullptr;
     LEXP_CUDA(cudaMalloc(&d_rs, 9 * HW * sizeof(int)));
     dim3 blk(128), grd((W + 127) / 128, H);
-    LEXP_LAUNCH(lexp_stats_rowsum, grd, blk, 0, c->stream, c->d_guide[mode], d_rs, H, W, c->R);
-    LEXP_LAUNCH(lexp_stats_finish, grd, blk, 0, c->stream, d_rs, c->d_statA[mode], c->d_statB[mode], c->d_statC[mode], H, W, c->R, (double)c->p.eps);
-    c->launches += 2;
-    if (c->p.energy_kind == 1) {
+    cudaError_t e = launch_aux(c, lexp_stats_rowsum, grd, blk, c->d_guide[mode], d_rs, H, W, c->R);
+    if (e == cudaSuccess)
+        e = launch_aux(c, lexp_stats_finish, grd, blk, d_rs, c->d_statA[mode], c->d_statB[mode], c->d_statC[mode], H, W, c->R, (double)c->p.eps);
+    if (e == cudaSuccess && c->p.energy_kind == 1) {
         if (!c->d_exi[mode] && cudaMalloc(&c->d_exi[mode], HW * sizeof(float4)) != cudaSuccess) { cudaFree(d_rs); return fail(LEXP_ERR_NOMEM, "ExI allocation failed"); }
         const float s_col = (float)(1.0 - (double)c->p.alpha);  // `I[m] * (1.0 - params.alpha)`, StereoEnergy.h:659
-        LEXP_LAUNCH(lexp_build_exi, grd, blk, 0, c->stream, c->d_guide[mode], c->d_exi[mode], H, W, s_col, c->p.alpha);
-        c->launches++;
+        e = launch_aux(c, lexp_build_exi, grd, blk, c->d_guide[mode], c->d_exi[mode], H, W, s_col, c->p.alpha);
     }
-    cudaError_t e = cudaGetLastError();
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     cudaFree(d_rs);
     if (e != cudaSuccess) return fail(LEXP_ERR_CUDA, std::string("statistics kernels: ") + cudaGetErrorString(e));
@@ -616,13 +714,9 @@ int lexp_set_image(lexp_ctx* c, int mode, const uint8_t* bgr, ptrdiff_t step) {
 int lexp_set_volume_host_ex(lexp_ctx* c, int mode, const float* vol, int transform) {
     if (!c || !vol || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
     { int rc = check_transform(mode, transform); if (rc) return rc; }
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    const int D = c->p.ndisp, H = c->p.height, W = c->p.width;
-    const size_t plane = (size_t)H * W;
-    int slab = (int)std::max<size_t>(8, std::min<size_t>((size_t)D, ((size_t)env_int("LEXP_UPLOAD_SLAB_MB", 512) << 20) / (plane * sizeof(float))));
-    slab = std::min(D, (slab + 7) / 8 * 8);
+    LEXP_ENTER(c);
+    const int D = c->p.ndisp, slab = upload_slab(c);
+    const size_t plane = (size_t)c->p.height * c->p.width;
     int* d_flag = nullptr;
     { int rc = alloc_volume(c, mode, &d_flag); if (rc) return rc; }
     float* stage = nullptr;
@@ -631,7 +725,7 @@ int lexp_set_volume_host_ex(lexp_ctx* c, int mode, const float* vol, int transfo
     const int tk = kernel_transform(mode, transform);
     for (int d_lo = 0; d_lo < D && e == cudaSuccess && rc == LEXP_OK; d_lo += slab) {
         const int nd = std::min(slab, D - d_lo);
-        e = cudaMemcpyAsync(stage, vol + (size_t)d_lo * plane, (size_t)nd * plane * sizeof(float), cudaMemcpyHostToDevice, c->stream);
+        e = h2d(c, stage, vol + (size_t)d_lo * plane, (size_t)nd * plane * sizeof(float));
         if (e != cudaSuccess) break;
         rc = ingest_slab(c, mode, stage, d_lo, nd, tk, d_flag);
     }
@@ -647,22 +741,18 @@ int lexp_set_volume_host_ex(lexp_ctx* c, int mode, const float* vol, int transfo
 int lexp_set_volume_file(lexp_ctx* c, int mode, const char* path, int transform) {
     if (!c || !path || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
     { int rc = check_transform(mode, transform); if (rc) return rc; }
-    const int D = c->p.ndisp, H = c->p.height, W = c->p.width;
-    const size_t plane = (size_t)H * W;
-    FILE* f = fopen(path, "rb");
+    const int D = c->p.ndisp;
+    const size_t plane = (size_t)c->p.height * c->p.width;
+    std::unique_ptr<FILE, int (*)(FILE*)> file(fopen(path, "rb"), fclose);
+    FILE* f = file.get();
     if (!f) return fail(LEXP_ERR_INVALID, std::string("cost volume file not found: ") + path);
-    if (fseek(f, 0, SEEK_END) != 0 || (unsigned long long)ftell(f) != (unsigned long long)D * plane * sizeof(float)) {
-        fclose(f);
+    if (fseek(f, 0, SEEK_END) != 0 || (unsigned long long)ftell(f) != (unsigned long long)D * plane * sizeof(float))
         return fail(LEXP_ERR_INVALID, std::string("cost volume file is not float[D][H][W] of this context's size: ") + path);
-    }
     rewind(f);
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    if (cudaSetDevice(c->p.device) != cudaSuccess) { fclose(f); return fail(LEXP_ERR_CUDA, "cudaSetDevice"); }
-    int slab = (int)std::max<size_t>(8, std::min<size_t>((size_t)D, ((size_t)env_int("LEXP_UPLOAD_SLAB_MB", 512) << 20) / (plane * sizeof(float))));
-    slab = std::min(D, (slab + 7) / 8 * 8);
+    LEXP_ENTER(c);
+    const int slab = upload_slab(c);
     int* d_flag = nullptr;
-    { int rc = alloc_volume(c, mode, &d_flag); if (rc) { fclose(f); return rc; } }
+    { int rc = alloc_volume(c, mode, &d_flag); if (rc) return rc; }
     float* stage = nullptr;
     float* host[2] = {nullptr, nullptr};
     cudaEvent_t copied[2] = {nullptr, nullptr};
@@ -678,12 +768,11 @@ int lexp_set_volume_file(lexp_ctx* c, int mode, const char* path, int transform)
         e = cudaEventSynchronize(copied[i]);   // the upload that last read this host buffer has finished (no-op the first time)
         if (e != cudaSuccess) break;
         if (fread(host[i], sizeof(float), (size_t)nd * plane, f) != (size_t)nd * plane) { rc = fail(LEXP_ERR_INVALID, std::string("short read: ") + path); break; }
-        e = cudaMemcpyAsync(stage, host[i], (size_t)nd * plane * sizeof(float), cudaMemcpyHostToDevice, c->stream);   // behind the previous slab's re-layout
+        e = h2d(c, stage, host[i], (size_t)nd * plane * sizeof(float));   // behind the previous slab's re-layout
         if (e == cudaSuccess) e = cudaEventRecord(copied[i], c->stream);
         if (e != cudaSuccess) break;
         rc = ingest_slab(c, mode, stage, d_lo, nd, tk, d_flag);
     }
-    fclose(f);
     if (e != cudaSuccess && rc == LEXP_OK) rc = fail(LEXP_ERR_CUDA, std::string("volume file upload: ") + cudaGetErrorString(e));
     const int rc2 = finish_volume(c, mode, d_flag);   // synchronises the stream
     cudaFree(stage);
@@ -694,13 +783,11 @@ int lexp_set_volume_file(lexp_ctx* c, int mode, const char* path, int transform)
 int lexp_set_volume_device_ex(lexp_ctx* c, int mode, const float* vol, int transform) {
     if (!c || !vol || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
     { int rc = check_transform(mode, transform); if (rc) return rc; }
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
     cudaPointerAttributes at;
     LEXP_CUDA(cudaPointerGetAttributes(&at, vol));
     if (at.type != cudaMemoryTypeDevice && at.type != cudaMemoryTypeManaged)
         return fail(LEXP_ERR_INVALID, "lexp_set_volume_device needs a device pointer");
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     // the caller's volume was produced on a stream this library does not know (e.g. torch's): the context's own stream is
     // non-blocking, so nothing orders its re-layout kernel behind that producer -- wait for the device once (one-time set-up call)
     LEXP_CUDA(cudaDeviceSynchronize());
@@ -717,19 +804,12 @@ int lexp_set_volume_device(lexp_ctx* c, int mode, const float* vol) { return lex
 int lexp_get_stats(lexp_ctx* c, int mode, float* out9) {
     if (!c || !out9 || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
     if (!c->d_statA[mode]) return fail(LEXP_ERR_STATE, "image not set");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     const size_t HW = (size_t)c->p.height * c->p.width;
-    float* d9 = nullptr;
-    LEXP_CUDA(cudaMalloc(&d9, 9 * HW * sizeof(float)));
-    LEXP_LAUNCH(lexp_stats_unpack, (unsigned)((HW + 255) / 256), 256, 0, c->stream, c->d_statA[mode], c->d_statB[mode], c->d_statC[mode], d9, HW);
-    c->launches++;
-    cudaError_t e = cudaStreamSynchronize(c->stream);
-    if (e == cudaSuccess) e = cudaMemcpy(out9, d9, 9 * HW * sizeof(float), cudaMemcpyDeviceToHost);
-    cudaFree(d9);
-    if (e != cudaSuccess) return fail(LEXP_ERR_CUDA, std::string("get_stats: ") + cudaGetErrorString(e));
-    return LEXP_OK;
+    return read_back(c, "get_stats", 9 * HW * sizeof(float), 0, out9, 9 * HW * sizeof(float), [&](char* d9) {
+        return launch_aux(c, lexp_stats_unpack, (unsigned)((HW + 255) / 256), 256, c->d_statA[mode], c->d_statB[mode], c->d_statC[mode],
+                          reinterpret_cast<float*>(d9), HW);
+    });
 }
 
 int lexp_plan_create(lexp_ctx* c, int n, const lexp_rect* filt, const lexp_rect* targ, lexp_plan** out_plan) {
@@ -738,8 +818,7 @@ int lexp_plan_create(lexp_ctx* c, int n, const lexp_rect* filt, const lexp_rect*
         int rc = check_rects(c, filt[i], targ[i]);
         if (rc) return rc;
     }
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     const int R = c->R;
     int ow_max = max_tile_ow(R);
     if (c->smem_cap)  // narrower tiles so that every work item fits the per-CTA shared-memory budget of the build
@@ -813,7 +892,7 @@ int lexp_plan_create(lexp_ctx* c, int n, const lexp_rect* filt, const lexp_rect*
     cudaError_t e = cudaMalloc(&pl->d_items, items.size() * sizeof(Item));
     if (e == cudaSuccess) e = cudaMalloc(&pl->d_planes, (size_t)n * sizeof(Plane4));
     // on the context's (non-blocking) stream, then synchronised: a legacy-stream cudaMemcpy is not ordered against the launches that read the items
-    if (e == cudaSuccess) e = cudaMemcpyAsync(pl->d_items, items.data(), items.size() * sizeof(Item), cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = h2d(c, pl->d_items, items.data(), items.size() * sizeof(Item));
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     if (e != cudaSuccess) {
         cudaFree(pl->d_items); cudaFree(pl->d_planes);
@@ -856,29 +935,13 @@ int lexp_plan_eval_device(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane
                           float* d_cost_image, ptrdiff_t step_bytes, int with_check) {
     if (!c || !pl || !planes || !d_cost_image || pl->ctx != c) return fail(LEXP_ERR_INVALID, "bad argument");
     if (step_bytes % 4 != 0 || step_bytes < (ptrdiff_t)c->p.width * 4) return fail(LEXP_ERR_INVALID, "bad row pitch");
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    const Plane4* dp = reinterpret_cast<const Plane4*>(planes);
-    if (!planes_on_device) {
-        LEXP_CUDA(cudaMemcpyAsync(pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
-        dp = pl->d_planes;
-        c->chain_ok = false;
-    }
-    return run_plan(c, pl, mode, dp, d_cost_image, step_bytes / 4, 0, with_check, nullptr, planes_on_device && c->overlap);
+    return eval_device(c, pl, mode, planes, planes_on_device, d_cost_image, step_bytes / 4, 0, with_check);
 }
 
 int lexp_plan_eval_device_tiles(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, int planes_on_device,
                                 float* d_tiles, int with_check) {
     if (!c || !pl || !planes || !d_tiles || pl->ctx != c) return fail(LEXP_ERR_INVALID, "bad argument");
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    const Plane4* dp = reinterpret_cast<const Plane4*>(planes);
-    if (!planes_on_device) {
-        LEXP_CUDA(cudaMemcpyAsync(pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
-        dp = pl->d_planes;
-        c->chain_ok = false;
-    }
-    return run_plan(c, pl, mode, dp, d_tiles, 0, 1, with_check, nullptr, planes_on_device && c->overlap);
+    return eval_device(c, pl, mode, planes, planes_on_device, d_tiles, 0, 1, with_check);
 }
 
 // Host planes in, per-call contiguous tiles out into HOST memory; blocking.  For the step-wise restructured loop
@@ -887,22 +950,12 @@ int lexp_plan_eval_device_tiles(lexp_ctx* c, lexp_plan* pl, int mode, const lexp
 // tile are contiguous in memory (full-line PCIe writes on the zero-copy path).
 int lexp_plan_eval_host_tiles(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, float* tiles, int with_check) {
     if (!c || !pl || !planes || !tiles || pl->ctx != c) return fail(LEXP_ERR_INVALID, "bad argument");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    LEXP_CUDA(cudaMemcpyAsync(pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
-    void* dptr = mapped_alias(tiles, (size_t)pl->sum_s * sizeof(float));
-    if (dptr) {  // registered (mapped) buffer: the kernel writes it directly
-        int rc = run_plan(c, pl, mode, pl->d_planes, reinterpret_cast<float*>(dptr), 0, 1, with_check);
-        if (rc) return rc;
-        LEXP_CUDA(cudaStreamSynchronize(c->stream));
-        return LEXP_OK;
-    }
-    // not a mapped buffer: compact device buffer, then one contiguous copy
+    LEXP_ENTER(c);
     const size_t nout = (size_t)pl->sum_s;
-    { int rc0 = ensure_compact(pl, nout); if (rc0) return rc0; }
-    int rc = run_plan(c, pl, mode, pl->d_planes, pl->d_compact, 0, 1, with_check);
-    if (rc) return rc;
+    // registered (mapped) buffer: the kernel writes it directly
+    float* d_direct = static_cast<float*>(mapped_alias(tiles, nout * sizeof(float)));
+    { int rc = eval_host(c, pl, mode, planes, d_direct, 0, 1, with_check); if (rc || d_direct) return rc; }
+    // not a mapped buffer: compact device buffer, then one contiguous copy
     bool part_locked = false;   // starts inside a page-locked registration that ends before the buffer does (mapped_alias said no)
 #ifndef LEXP_EMU
     cudaPointerAttributes pa{};
@@ -910,12 +963,12 @@ int lexp_plan_eval_host_tiles(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_p
     cudaGetLastError();
 #endif
     if (part_locked) {   // the driver rejects a copy that runs past the end of the registration: bounce through the pinned mirror
-        LEXP_CUDA(cudaMemcpyAsync(pl->h_compact, pl->d_compact, nout * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+        LEXP_CUDA(d2h(c, pl->h_compact, pl->d_compact, nout * sizeof(float)));
         LEXP_CUDA(cudaStreamSynchronize(c->stream));
         memcpy(tiles, pl->h_compact, nout * sizeof(float));
         return LEXP_OK;
     }
-    LEXP_CUDA(cudaMemcpyAsync(tiles, pl->d_compact, nout * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    LEXP_CUDA(d2h(c, tiles, pl->d_compact, nout * sizeof(float)));
     LEXP_CUDA(cudaStreamSynchronize(c->stream));
     return LEXP_OK;
 }
@@ -923,32 +976,19 @@ int lexp_plan_eval_host_tiles(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_p
 int lexp_plan_eval_host(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, float* cost_image,
                         ptrdiff_t step_bytes, int with_check) {
     if (!c || !pl || !planes || !cost_image || pl->ctx != c) return fail(LEXP_ERR_INVALID, "bad argument");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    {   // zero-copy path: the caller's image is page-locked + mapped (lexp_host_register)
-        // the calls write rows t.y .. t.y + t.height - 1 of the image: the range that must be mapped spans them all
-        int y_lo = INT_MAX, y_hi = -1, x_hi = 0;
-        for (const lexp_rect& t : pl->targ) { y_lo = std::min(y_lo, t.y); y_hi = std::max(y_hi, t.y + t.height - 1); x_hi = std::max(x_hi, t.x + t.width); }
-        char* lo = reinterpret_cast<char*>(cost_image) + (ptrdiff_t)y_lo * step_bytes;
-        const size_t span = step_bytes > 0 && y_hi >= y_lo ? (size_t)(y_hi - y_lo) * (size_t)step_bytes + (size_t)x_hi * sizeof(float) : 0;
-        void* dlo = span ? mapped_alias(lo, span) : nullptr;
-        void* dptr = dlo ? static_cast<char*>(dlo) - (ptrdiff_t)y_lo * step_bytes : nullptr;
-        if (dptr) {
-            if (step_bytes % 4 != 0) return fail(LEXP_ERR_INVALID, "bad row pitch");
-            LEXP_CUDA(cudaMemcpyAsync(pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
-            int rc = run_plan(c, pl, mode, pl->d_planes, reinterpret_cast<float*>(dptr), step_bytes / 4, 0, with_check);
-            if (rc) return rc;
-            LEXP_CUDA(cudaStreamSynchronize(c->stream));
-            return LEXP_OK;
-        }
-    }   // not a mapped buffer: staged path below
-    const size_t nout = (size_t)pl->sum_s;
-    { int rc0 = ensure_compact(pl, nout); if (rc0) return rc0; }
-    LEXP_CUDA(cudaMemcpyAsync(pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
-    int rc = run_plan(c, pl, mode, pl->d_planes, pl->d_compact, 0, 1, with_check);
-    if (rc) return rc;
-    LEXP_CUDA(cudaMemcpyAsync(pl->h_compact, pl->d_compact, nout * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    LEXP_ENTER(c);
+    // zero-copy path: the caller's image is page-locked + mapped (lexp_host_register).  The calls write rows
+    // t.y .. t.y + t.height - 1 of the image: the range that must be mapped spans them all
+    int y_lo = INT_MAX, y_hi = -1, x_hi = 0;
+    for (const lexp_rect& t : pl->targ) { y_lo = std::min(y_lo, t.y); y_hi = std::max(y_hi, t.y + t.height - 1); x_hi = std::max(x_hi, t.x + t.width); }
+    char* lo = reinterpret_cast<char*>(cost_image) + (ptrdiff_t)y_lo * step_bytes;
+    const size_t span = step_bytes > 0 && y_hi >= y_lo ? (size_t)(y_hi - y_lo) * (size_t)step_bytes + (size_t)x_hi * sizeof(float) : 0;
+    void* dlo = span ? mapped_alias(lo, span) : nullptr;
+    float* d_direct = dlo ? reinterpret_cast<float*>(static_cast<char*>(dlo) - (ptrdiff_t)y_lo * step_bytes) : nullptr;
+    if (d_direct && step_bytes % 4 != 0) return fail(LEXP_ERR_INVALID, "bad row pitch");
+    { int rc = eval_host(c, pl, mode, planes, d_direct, step_bytes / 4, 0, with_check); if (rc || d_direct) return rc; }
+    // not a mapped buffer: staged through the compact buffer and its pinned mirror
+    LEXP_CUDA(d2h(c, pl->h_compact, pl->d_compact, (size_t)pl->sum_s * sizeof(float)));
     LEXP_CUDA(cudaStreamSynchronize(c->stream));
     // scatter the per-call tiles into the caller's image: costs(targetRect) only (CostVolumeEnergy.h:169-171)
     for (int i = 0; i < pl->ncalls; i++) {
@@ -967,11 +1007,7 @@ int lexp_eval_batch(lexp_ctx* c, int mode, int n, const lexp_rect* filt, const l
     lexp_plan* pl = nullptr;
     int rc = lexp_plan_create(c, n, filt, targ, &pl);
     if (rc) return rc;
-    rc = lexp_plan_eval_host(c, pl, mode, planes, cost_image, step_bytes, with_check);
-    std::string keep = g_err;
-    lexp_plan_destroy(pl);
-    g_err = keep;
-    return rc;
+    return eval_host_once(c, pl, mode, planes, cost_image, step_bytes, with_check);
 }
 
 namespace {
@@ -983,9 +1019,7 @@ int run_combined(lexp_ctx* c, const std::vector<lexp_ctx::CellReq*>& reqs) {
     size_t nitems = 0, nout = 0, smem = 0;
     for (auto* r : reqs) { nitems += r->pl->h_items.size(); nout += (size_t)r->pl->sum_s; smem = std::max(smem, r->pl->smem); }
     if (nout > 0x7fffffffULL) return fail(LEXP_ERR_INVALID, "combined output too large");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     lexp_ctx::CombBuf& b = c->cb[c->cb_next];
     c->cb_next ^= 1;
     // the callers of the batch that used this buffer two batches ago must have copied their tiles out
@@ -1028,8 +1062,8 @@ int run_combined(lexp_ctx* c, const std::vector<lexp_ctx::CellReq*>& reqs) {
         const lexp_plane& p = reqs[i]->plane;
         b.h_planes[i] = Plane4{p.a, p.b, p.c, p.v};
     }
-    LEXP_CUDA(cudaMemcpyAsync(b.d_items, b.h_items, nitems * sizeof(Item), cudaMemcpyHostToDevice, c->stream));
-    LEXP_CUDA(cudaMemcpyAsync(b.d_planes, b.h_planes, reqs.size() * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
+    LEXP_CUDA(h2d(c, b.d_items, b.h_items, nitems * sizeof(Item)));
+    LEXP_CUDA(h2d(c, b.d_planes, b.h_planes, reqs.size() * sizeof(Plane4)));
     lexp_plan batch;  // a view: nothing in it is owned
     batch.ctx = c;
     batch.ncalls = (int)reqs.size();
@@ -1080,11 +1114,7 @@ int lexp_eval_cell(lexp_ctx* c, int mode, const lexp_rect* filt, const lexp_rect
             pl = ins.first->second;
         } else if (c->cell_plans.size() > 200000) {  // unbounded callers (initCurrentFast with a labeling: one rect per pixel)
             c->cell_plans.erase(ins.first);
-            int rc2 = lexp_plan_eval_host(c, pl, mode, plane, base, step_bytes, with_check);
-            std::string keep = g_err;
-            lexp_plan_destroy(pl);
-            g_err = keep;
-            return rc2;
+            return eval_host_once(c, pl, mode, plane, base, step_bytes, with_check);
         }
     }
     if (!c->combine || mode < 0 || mode > 1) return lexp_plan_eval_host(c, pl, mode, plane, base, step_bytes, with_check);
@@ -1187,9 +1217,8 @@ void* lexp_stream(lexp_ctx* c) { return c ? (void*)c->stream : nullptr; }
 
 int lexp_set_stream(lexp_ctx* c, void* s) {
     if (!c) return fail(LEXP_ERR_INVALID, "null ctx");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
+    c->chain_ok = false;   // the new stream's last operation is unknown: the next fused launch is an ordinary one
     // no synchronisation here (the call must be legal while the caller captures a CUDA graph): ordering between the
     // old and the new stream is the caller's business
     if (c->own_stream) { cudaStreamSynchronize(c->stream); cudaStreamDestroy(c->stream); c->own_stream = false; }
@@ -1209,39 +1238,31 @@ int lexp_set_overlap(lexp_ctx* c, int on) {
 // ---- PatchMatch phase on the device (FastGCStereo.h:94-157 with doGC == false) ---------------------------------------------
 int lexp_pm_begin(lexp_ctx* c, int mode, const float* cost, const lexp_plane* labeling) {
     if (!c || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     const size_t HW = (size_t)c->p.height * c->p.width;
     if (!c->d_cur_cost[mode]) LEXP_CUDA(cudaMalloc(&c->d_cur_cost[mode], HW * sizeof(float)));
     if (!c->d_cur_label[mode]) LEXP_CUDA(cudaMalloc(&c->d_cur_label[mode], HW * sizeof(float4)));
     if (!c->d_flags[mode]) {
         LEXP_CUDA(cudaMalloc(&c->d_flags[mode], (kMaxPeers + 2) * sizeof(int)));   // + epoch base + error flag
-        LEXP_CUDA(cudaMemsetAsync(c->d_flags[mode], 0, (kMaxPeers + 2) * sizeof(int), c->stream));   // epochs only grow: never reset while peers run
+        LEXP_CUDA(memset0(c, c->d_flags[mode], (kMaxPeers + 2) * sizeof(int)));   // epochs only grow: never reset while peers run
     }
-    if (cost) LEXP_CUDA(cudaMemcpyAsync(c->d_cur_cost[mode], cost, HW * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-    else {
-        LEXP_LAUNCH(lexp_fill_f32, c->num_sms * 4, 256, 0, c->stream, c->d_cur_cost[mode], HW, __builtin_inff());   // currentCost_ = INFINITY (:137)
-        LEXP_CUDA(cudaGetLastError());
-        c->launches++;
-    }
-    if (labeling) LEXP_CUDA(cudaMemcpyAsync(c->d_cur_label[mode], labeling, HW * sizeof(float4), cudaMemcpyHostToDevice, c->stream));
-    else LEXP_CUDA(cudaMemsetAsync(c->d_cur_label[mode], 0, HW * sizeof(float4), c->stream));
+    if (cost) LEXP_CUDA(h2d(c, c->d_cur_cost[mode], cost, HW * sizeof(float)));
+    else LEXP_CUDA(launch_aux(c, lexp_fill_f32, c->num_sms * 4, 256, c->d_cur_cost[mode], HW, __builtin_inff()));   // currentCost_ = INFINITY (:137)
+    if (labeling) LEXP_CUDA(h2d(c, c->d_cur_label[mode], labeling, HW * sizeof(float4)));
+    else LEXP_CUDA(memset0(c, c->d_cur_label[mode], HW * sizeof(float4)));
     if (cost || labeling) LEXP_CUDA(cudaStreamSynchronize(c->stream));  // the host buffers may be pageable
     return LEXP_OK;
 }
 
 int lexp_pm_get(lexp_ctx* c, int mode, float* cost, lexp_plane* labeling) {
     if (!c || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_cur_cost[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    LEXP_ENTER(c);
     const size_t HW = (size_t)c->p.height * c->p.width;
-    if (cost) LEXP_CUDA(cudaMemcpyAsync(cost, c->d_cur_cost[mode], HW * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    if (labeling) LEXP_CUDA(cudaMemcpyAsync(labeling, c->d_cur_label[mode], HW * sizeof(float4), cudaMemcpyDeviceToHost, c->stream));
+    if (cost) LEXP_CUDA(d2h(c, cost, c->d_cur_cost[mode], HW * sizeof(float)));
+    if (labeling) LEXP_CUDA(d2h(c, labeling, c->d_cur_label[mode], HW * sizeof(float4)));
     int err = 0;
-    LEXP_CUDA(cudaMemcpyAsync(&err, c->d_flags[mode] + kMaxPeers + 1, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    LEXP_CUDA(d2h(c, &err, c->d_flags[mode] + kMaxPeers + 1, sizeof(int)));
     LEXP_CUDA(cudaStreamSynchronize(c->stream));
     if (err == 2) return fail(LEXP_ERR_STATE, "a graph-cut move stopped at its round limit: the state is not the result of minimum cuts");
     if (err) return fail(LEXP_ERR_STATE, "a wait for a peer rank's group epoch timed out (multi-GPU cell shard): the state is incomplete");
@@ -1250,7 +1271,7 @@ int lexp_pm_get(lexp_ctx* c, int mode, float* cost, lexp_plane* labeling) {
 
 int lexp_pm_device_state(lexp_ctx* c, int mode, float** d_cost, lexp_plane** d_labeling) {
     if (!c || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_cur_cost[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
     if (d_cost) *d_cost = c->d_cur_cost[mode];
     if (d_labeling) *d_labeling = reinterpret_cast<lexp_plane*>(c->d_cur_label[mode]);
     return LEXP_OK;
@@ -1268,11 +1289,9 @@ int lexp_plan_set_units(lexp_plan* pl, const lexp_rect* units, const int* cell_i
             return fail(LEXP_ERR_INVALID, "unitRegion outside the image");
         h[i] = CallInfo{u.x, u.y, u.width, u.height, pl->items_per_call[i] * kWarpsE, cell_ids ? cell_ids[i] : i, pl->items_per_call[i], 0};
     }
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     if (!pl->d_calls) LEXP_CUDA(cudaMalloc(&pl->d_calls, (size_t)pl->ncalls * sizeof(CallInfo)));
-    LEXP_CUDA(cudaMemcpyAsync(pl->d_calls, h.data(), h.size() * sizeof(CallInfo), cudaMemcpyHostToDevice, c->stream));   // stream-ordered (see lexp_plan_create)
+    LEXP_CUDA(h2d(c, pl->d_calls, h.data(), h.size() * sizeof(CallInfo)));   // stream-ordered (see lexp_plan_create)
     LEXP_CUDA(cudaStreamSynchronize(c->stream));
     if (pl->sync_off < 0) {   // a slice of the context's synchronisation arena (offsets survive a re-allocation of the arena)
         const size_t need = ((size_t)pl->ncalls + 1) * sizeof(CellSync);
@@ -1280,7 +1299,7 @@ int lexp_plan_set_units(lexp_plan* pl, const lexp_rect* units, const int* cell_i
             const size_t cap = std::max<size_t>(2 * c->sync_cap, std::max<size_t>(1 << 20, c->sync_used + need));
             char* na = nullptr;
             LEXP_CUDA(cudaMalloc(&na, cap));
-            LEXP_CUDA(cudaMemsetAsync(na, 0, cap, c->stream));
+            LEXP_CUDA(memset0(c, na, cap));
             LEXP_CUDA(cudaStreamSynchronize(c->stream));
             cudaFree(c->d_sync_arena);   // the stream is idle (synchronised above); the records are zeroed before every iteration anyway
             c->d_sync_arena = na; c->sync_cap = cap;
@@ -1295,10 +1314,8 @@ int lexp_plan_set_units(lexp_plan* pl, const lexp_rect* units, const int* cell_i
 // are issued -- not between groups, so that all launches of an iteration form one programmatic-dependent-launch chain.
 int lexp_pm_reset_sync(lexp_ctx* c) {
     if (!c) return fail(LEXP_ERR_INVALID, "null ctx");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    if (c->sync_used) LEXP_CUDA(cudaMemsetAsync(c->d_sync_arena, 0, c->sync_used, c->stream));
+    LEXP_ENTER(c);
+    if (c->sync_used) LEXP_CUDA(memset0(c, c->d_sync_arena, c->sync_used));
     return LEXP_OK;
 }
 
@@ -1308,19 +1325,14 @@ int lexp_plan_pm_step_ex(lexp_ctx* c, lexp_plan* pl, int mode, int step_index, i
     if (kind < LEXP_PROP_LIST || kind > LEXP_PROP_RANDOM || m < 0 || m > 120) return fail(LEXP_ERR_INVALID, "bad proposer kind / m");
     if (kind == LEXP_PROP_LIST && !planes) return fail(LEXP_ERR_INVALID, "LEXP_PROP_LIST needs planes");
     if (!pl->d_calls || pl->sync_off < 0) return fail(LEXP_ERR_STATE, "lexp_plan_set_units has not been called for this plan");
-    if (!c->d_cur_cost[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
     if (c->p.energy_kind != 0) return fail(LEXP_ERR_INVALID, "the device PatchMatch phase is implemented for the cost-volume energy");
     if (publish_epoch < 0 || (wait_mask >> kMaxPeers) || (wait_mask && !wait_epochs)) return fail(LEXP_ERR_INVALID, "bad epoch / mask");
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    const Plane4* dp = nullptr;
+    LEXP_ENTER(c);
+    const Plane4* dp = nullptr;   // the other kinds: the device proposers generate the planes
     if (kind == LEXP_PROP_LIST) {
-        dp = reinterpret_cast<const Plane4*>(planes);
-        if (!planes_on_device) {
-            LEXP_CUDA(cudaMemcpyAsync(pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
-            dp = pl->d_planes;
-            c->chain_ok = false;
-        }
+        dp = stage_planes(c, pl, planes, planes_on_device);
+        if (!dp) return LEXP_ERR_CUDA;
     }
     PmArgs pm{(flags & LEXP_PM_INIT) ? 2 : 1, kind, m, step_index, (unsigned long long)seed, reinterpret_cast<Plane4*>(d_planes_out),
               publish_epoch, {0, 0, 0, 0, 0, 0, 0, 0}, wait_mask};
@@ -1336,13 +1348,9 @@ int lexp_plan_pm_step(lexp_ctx* c, lexp_plan* pl, int mode, int step_index, int 
 
 int lexp_pm_advance_epoch(lexp_ctx* c, int mode, int delta) {
     if (!c || mode < 0 || mode > 1 || delta < 0) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_flags[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    LEXP_LAUNCH(lexp_add_i32, 1, 1, 0, c->stream, c->d_flags[mode] + kMaxPeers, delta);
-    LEXP_CUDA(cudaGetLastError());
-    c->launches++;
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    LEXP_ENTER(c);
+    LEXP_CUDA(launch_aux(c, lexp_add_i32, 1, 1, c->d_flags[mode] + kMaxPeers, delta));
     return LEXP_OK;
 }
 
@@ -1355,9 +1363,7 @@ int ensure_coef(lexp_ctx* c, int mode) {
     const int H = c->p.height, W = c->p.width;
     if (!c->d_coef[mode]) LEXP_CUDA(cudaMalloc(&c->d_coef[mode], (size_t)H * W * sizeof(float4)));
     dim3 blk(128), grd((W + 127) / 128, H);
-    LEXP_LAUNCH(lexp_smooth_coeff_kernel, grd, blk, 0, c->stream, c->d_guide[mode], c->d_coef[mode], H, W, c->sm_omega, c->sm_eps);
-    LEXP_CUDA(cudaGetLastError());
-    c->launches++;
+    LEXP_CUDA(launch_aux(c, lexp_smooth_coeff_kernel, grd, blk, c->d_guide[mode], c->d_coef[mode], H, W, c->sm_omega, c->sm_eps));
     c->coef_valid[mode] = true;
     return LEXP_OK;
 }
@@ -1369,22 +1375,29 @@ int upload_gc_cells(lexp_ctx* c, int n, const lexp_rect* regions, GcCell** d_cel
         at += (long long)regions[i].width * regions[i].height;
     }
     LEXP_CUDA(cudaMalloc(d_cells, (size_t)n * sizeof(GcCell)));
-    LEXP_CUDA(cudaMemcpyAsync(*d_cells, h.data(), (size_t)n * sizeof(GcCell), cudaMemcpyHostToDevice, c->stream));
+    LEXP_CUDA(h2d(c, *d_cells, h.data(), (size_t)n * sizeof(GcCell)));
     LEXP_CUDA(cudaStreamSynchronize(c->stream));   // h is pageable and local
     *nodes = at;
     return LEXP_OK;
 }
-}  // namespace
+// proposalCost image of the view and the graph-cut cells of the plan (lexp_plan_init_step, lexp_plan_gc_step)
+int ensure_gc_plan_state(lexp_ctx* c, lexp_plan* pl, int mode) {
+    if (!c->d_prop_cost[mode]) LEXP_CUDA(cudaMalloc(&c->d_prop_cost[mode], (size_t)c->p.height * c->p.width * sizeof(float)));
+    if (pl->d_gc_cells) return LEXP_OK;
+    int rc = upload_gc_cells(c, pl->ncalls, pl->targ.data(), &pl->d_gc_cells, &pl->gc_nodes);
+    if (rc) return rc;
+    for (const lexp_rect& t : pl->targ) pl->gc_max_nodes = std::max(pl->gc_max_nodes, t.width * t.height);
+    return LEXP_OK;
+}
 
-namespace {
-void gc_phase(int phase, lexp_ctx* c, lexp_plan* pl, const GcParams& gp, const GcPhaseCtl& ctl, int cur) {   // (no template: C linkage block)
-#define LEXP_GC_PHASE_CASE(PH) case PH: LEXP_LAUNCH((lexp_gc_phase_kernel<PH>), pl->gc_nblocks, kGcPhaseThreads, 0, c->stream, gp, ctl, cur); break;
+cudaError_t gc_phase(int phase, lexp_ctx* c, lexp_plan* pl, const GcParams& gp, const GcPhaseCtl& ctl, int cur) {   // (no template: C linkage block)
+#define LEXP_GC_PHASE_CASE(PH) case PH: return launch_aux(c, lexp_gc_phase_kernel<PH>, pl->gc_nblocks, kGcPhaseThreads, gp, ctl, cur);
     switch (phase) {
         LEXP_GC_PHASE_CASE(GC_PH_BUILD) LEXP_GC_PHASE_CASE(GC_PH_GATHER) LEXP_GC_PHASE_CASE(GC_PH_CLEAR) LEXP_GC_PHASE_CASE(GC_PH_RELAX)
         LEXP_GC_PHASE_CASE(GC_PH_ACTIVE) LEXP_GC_PHASE_CASE(GC_PH_PUSH) LEXP_GC_PHASE_CASE(GC_PH_RELABEL) LEXP_GC_PHASE_CASE(GC_PH_APPLY)
     }
 #undef LEXP_GC_PHASE_CASE
-    c->launches++;
+    return cudaErrorInvalidValue;
 }
 // block map + control block of the phase kernels (once per plan)
 int ensure_gc_phase_plan(lexp_ctx* c, lexp_plan* pl) {
@@ -1401,7 +1414,7 @@ int ensure_gc_phase_plan(lexp_ctx* c, lexp_plan* pl) {
     char* d_ctl = nullptr;
     cudaError_t e = cudaMalloc(&d_blocks, blocks.size() * sizeof(GcBlock));
     if (e == cudaSuccess) e = cudaMalloc(&d_ctl, ints * sizeof(int) + 2 * blocks.size() * sizeof(double));
-    if (e == cudaSuccess) e = cudaMemcpyAsync(d_blocks, blocks.data(), blocks.size() * sizeof(GcBlock), cudaMemcpyHostToDevice, c->stream);
+    if (e == cudaSuccess) e = h2d(c, d_blocks, blocks.data(), blocks.size() * sizeof(GcBlock));
     if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);   // `blocks` is local
     if (e != cudaSuccess) {   // both buffers or neither
         cudaFree(d_blocks); cudaFree(d_ctl); pl->gc_nblocks = 0;
@@ -1421,47 +1434,42 @@ int run_gc_phases(lexp_ctx* c, lexp_plan* pl, const GcParams& gp, double* d_flow
     ctl.blocks = pl->d_gc_blocks; ctl.done = ibase; ctl.active = ibase + pl->ncalls; ctl.g_flags = ibase + 2 * pl->ncalls;
     ctl.konst_part = reinterpret_cast<double*>(pl->d_gc_ctl + ints * sizeof(int)); ctl.sink_part = ctl.konst_part + pl->gc_nblocks;
     ctl.ncells = pl->ncalls;
-    LEXP_CUDA(cudaMemsetAsync(ibase, 0, ints * sizeof(int), c->stream));
-    gc_phase(GC_PH_BUILD, c, pl, gp, ctl, 0);
+    LEXP_CUDA(memset0(c, ibase, ints * sizeof(int)));
+    LEXP_CUDA(gc_phase(GC_PH_BUILD, c, pl, gp, ctl, 0));
     auto flag = [&](int which, int* out) -> cudaError_t {   // read a decision flag back (and leave it cleared for the next use)
-        cudaError_t e = cudaMemcpyAsync(c->h_gc_flags + which, ctl.g_flags + which, sizeof(int), cudaMemcpyDeviceToHost, c->stream);
-        if (e == cudaSuccess) e = cudaMemsetAsync(ctl.g_flags + which, 0, sizeof(int), c->stream);
+        cudaError_t e = d2h(c, c->h_gc_flags + which, ctl.g_flags + which, sizeof(int));
+        if (e == cudaSuccess) e = memset0(c, ctl.g_flags + which, sizeof(int));
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
         *out = c->h_gc_flags[which];
         return e;
     };
     int cur = 0, rounds = 0;
     for (;;) {
-        gc_phase(GC_PH_GATHER, c, pl, gp, ctl, cur);    // global relabelling: pending pushes, then exact distances by relaxation passes
-        gc_phase(GC_PH_CLEAR, c, pl, gp, ctl, cur);
+        LEXP_CUDA(gc_phase(GC_PH_GATHER, c, pl, gp, ctl, cur));    // global relabelling: pending pushes, then exact distances by relaxation passes
+        LEXP_CUDA(gc_phase(GC_PH_CLEAR, c, pl, gp, ctl, cur));
         for (int changed = 1; changed;) {
-            for (int pass = 0; pass < 8; pass++) gc_phase(GC_PH_RELAX, c, pl, gp, ctl, cur);
+            for (int pass = 0; pass < 8; pass++) LEXP_CUDA(gc_phase(GC_PH_RELAX, c, pl, gp, ctl, cur));
             LEXP_CUDA(flag(0, &changed));
         }
-        gc_phase(GC_PH_ACTIVE, c, pl, gp, ctl, cur);
-        LEXP_LAUNCH(lexp_gc_phase_decide, (pl->ncalls + 127) / 128, 128, 0, c->stream, ctl);
-        c->launches++;
+        LEXP_CUDA(gc_phase(GC_PH_ACTIVE, c, pl, gp, ctl, cur));
+        LEXP_CUDA(launch_aux(c, lexp_gc_phase_decide, (pl->ncalls + 127) / 128, 128, ctl));
         int any_active = 0;
         LEXP_CUDA(flag(1, &any_active));
         if (!any_active) break;
         if (rounds >= c->gc_max_rounds) {   // bounded like every loop of the device path; reported by lexp_pm_get
             const int two = 2;
-            LEXP_CUDA(cudaMemcpyAsync(gp.err_flag, &two, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+            LEXP_CUDA(h2d(c, gp.err_flag, &two, sizeof(int)));
             LEXP_CUDA(cudaStreamSynchronize(c->stream));
             break;
         }
         for (int r = 0; r < c->gc_relabel_every; r++, rounds++) {
-            gc_phase(GC_PH_PUSH, c, pl, gp, ctl, cur);
-            gc_phase(GC_PH_RELABEL, c, pl, gp, ctl, cur);
+            LEXP_CUDA(gc_phase(GC_PH_PUSH, c, pl, gp, ctl, cur));
+            LEXP_CUDA(gc_phase(GC_PH_RELABEL, c, pl, gp, ctl, cur));
             cur ^= 1;
         }
     }
-    gc_phase(GC_PH_APPLY, c, pl, gp, ctl, cur);
-    if (d_flows_out) {
-        LEXP_LAUNCH(lexp_gc_phase_flows, (pl->ncalls + 127) / 128, 128, 0, c->stream, ctl, pl->gc_nblocks, d_flows_out);
-        c->launches++;
-    }
-    LEXP_CUDA(cudaGetLastError());
+    LEXP_CUDA(gc_phase(GC_PH_APPLY, c, pl, gp, ctl, cur));
+    if (d_flows_out) LEXP_CUDA(launch_aux(c, lexp_gc_phase_flows, (pl->ncalls + 127) / 128, 128, ctl, pl->gc_nblocks, d_flows_out));
     return LEXP_OK;
 }
 }  // namespace
@@ -1477,35 +1485,23 @@ int lexp_set_smoothness(lexp_ctx* c, float lambda, float omega, float th_smooth,
 
 int lexp_get_smooth_coeff(lexp_ctx* c, int mode, float* out8) {
     if (!c || !out8 || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     { int rc = ensure_coef(c, mode); if (rc) return rc; }
     const int H = c->p.height, W = c->p.width;
-    const size_t HW = (size_t)H * W;
-    float* d8 = nullptr;
-    LEXP_CUDA(cudaMalloc(&d8, 8 * HW * sizeof(float)));
-    dim3 blk(128), grd((W + 127) / 128, H);
-    LEXP_LAUNCH(lexp_smooth_coeff_unpack, grd, blk, 0, c->stream, c->d_coef[mode], d8, H, W);
-    c->launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out8, d8, 8 * HW * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cudaFree(d8);
-    if (e != cudaSuccess) return fail(LEXP_ERR_CUDA, std::string("get_smooth_coeff: ") + cudaGetErrorString(e));
-    return LEXP_OK;
+    const size_t bytes = 8 * (size_t)H * W * sizeof(float);
+    return read_back(c, "get_smooth_coeff", bytes, 0, out8, bytes, [&](char* d8) {
+        return launch_aux(c, lexp_smooth_coeff_unpack, dim3((W + 127) / 128, H), 128, c->d_coef[mode], reinterpret_cast<float*>(d8), H, W);
+    });
 }
 
 int lexp_pairwise_terms(lexp_ctx* c, int mode, int n, const lexp_rect* regions, const lexp_plane* planes, float* out_host) {
     if (!c || !regions || !planes || !out_host || n <= 0 || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_cur_label[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
     const int H = c->p.height, W = c->p.width;
     for (int i = 0; i < n; i++)
         if (regions[i].width <= 0 || regions[i].height <= 0 || regions[i].x < 0 || regions[i].y < 0 || regions[i].x + regions[i].width > W ||
             regions[i].y + regions[i].height > H) return fail(LEXP_ERR_INVALID, "region outside the image");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     { int rc = ensure_coef(c, mode); if (rc) return rc; }
     GcCell* d_cells = nullptr;
     Plane4* d_planes = nullptr;
@@ -1516,13 +1512,10 @@ int lexp_pairwise_terms(lexp_ctx* c, int mode, int n, const lexp_rect* regions, 
     if (rc == LEXP_OK) {
         e = cudaMalloc(&d_planes, (size_t)n * sizeof(Plane4));
         if (e == cudaSuccess) e = cudaMalloc(&d_out, (size_t)nodes * 12 * sizeof(float));
-        if (e == cudaSuccess) e = cudaMemcpyAsync(d_planes, planes, (size_t)n * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream);
-        if (e == cudaSuccess) {
-            LEXP_LAUNCH(lexp_pairwise_kernel, n, 256, 0, c->stream, d_cells, d_planes, c->d_cur_label[mode], c->d_coef[mode], d_out, H, W, c->sm_lambda, c->sm_th);
-            c->launches++;
-            e = cudaGetLastError();
-        }
-        if (e == cudaSuccess) e = cudaMemcpyAsync(out_host, d_out, (size_t)nodes * 12 * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
+        if (e == cudaSuccess) e = h2d(c, d_planes, planes, (size_t)n * sizeof(Plane4));
+        if (e == cudaSuccess)
+            e = launch_aux(c, lexp_pairwise_kernel, n, 256, d_cells, d_planes, c->d_cur_label[mode], c->d_coef[mode], d_out, H, W, c->sm_lambda, c->sm_th);
+        if (e == cudaSuccess) e = d2h(c, out_host, d_out, (size_t)nodes * 12 * sizeof(float));
         if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
     }
     cudaFree(d_cells); cudaFree(d_planes); cudaFree(d_out);
@@ -1533,48 +1526,26 @@ int lexp_pairwise_terms(lexp_ctx* c, int mode, int n, const lexp_rect* regions, 
 
 int lexp_plan_init_step(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, int planes_on_device) {
     if (!c || !pl || pl->ctx != c || !planes || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_cur_cost[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    c->chain_ok = false;   // copies / other kernels around the fused launch: it is an ordinary one
-    const int H = c->p.height, W = c->p.width;
-    if (!c->d_prop_cost[mode]) LEXP_CUDA(cudaMalloc(&c->d_prop_cost[mode], (size_t)H * W * sizeof(float)));
-    if (!pl->d_gc_cells) {
-        int rc = upload_gc_cells(c, pl->ncalls, pl->targ.data(), &pl->d_gc_cells, &pl->gc_nodes);
-        if (rc) return rc;
-        for (const lexp_rect& t : pl->targ) pl->gc_max_nodes = std::max(pl->gc_max_nodes, t.width * t.height);
-    }
-    const Plane4* dp = reinterpret_cast<const Plane4*>(planes);
-    if (!planes_on_device) {
-        LEXP_CUDA(cudaMemcpyAsync(pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
-        dp = pl->d_planes;
-    }
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    LEXP_ENTER(c);
+    { int rc = ensure_gc_plan_state(c, pl, mode); if (rc) return rc; }
+    const Plane4* dp = stage_planes(c, pl, planes, planes_on_device);
+    if (!dp) return LEXP_ERR_CUDA;
+    const int W = c->p.width;
     { int rc = run_plan(c, pl, mode, dp, c->d_prop_cost[mode], W, 0, 1); if (rc) return rc; }   // ComputeUnaryPotential (:111)
-    c->chain_ok = false;
-    LEXP_LAUNCH(lexp_gc_assign_kernel, pl->ncalls, 256, 0, c->stream, pl->d_gc_cells, dp, c->d_prop_cost[mode], c->d_cur_cost[mode], c->d_cur_label[mode], W);
-    LEXP_CUDA(cudaGetLastError());
-    c->launches++;
+    LEXP_CUDA(launch_aux(c, lexp_gc_assign_kernel, pl->ncalls, 256, pl->d_gc_cells, dp, c->d_prop_cost[mode], c->d_cur_cost[mode], c->d_cur_label[mode], W));
     return LEXP_OK;
 }
 
 int lexp_get_disparities(lexp_ctx* c, int mode, float* out_host) {
     if (!c || !out_host || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_cur_label[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    LEXP_ENTER(c);
     const int H = c->p.height, W = c->p.width;
-    float* d = nullptr;
-    LEXP_CUDA(cudaMalloc(&d, (size_t)H * W * sizeof(float)));
-    dim3 blk(128), grd((W + 127) / 128, H);
-    LEXP_LAUNCH(lexp_disparity_kernel, grd, blk, 0, c->stream, c->d_cur_label[mode], d, H, W);
-    c->launches++;
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(out_host, d, (size_t)H * W * sizeof(float), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cudaFree(d);
-    if (e != cudaSuccess) return fail(LEXP_ERR_CUDA, std::string("lexp_get_disparities: ") + cudaGetErrorString(e));
-    return LEXP_OK;
+    const size_t bytes = (size_t)H * W * sizeof(float);
+    return read_back(c, "lexp_get_disparities", bytes, 0, out_host, bytes, [&](char* d) {
+        return launch_aux(c, lexp_disparity_kernel, dim3((W + 127) / 128, H), 128, c->d_cur_label[mode], reinterpret_cast<float*>(d), H, W);
+    });
 }
 
 // cvutils::io::save_pfm_file (Utilities.hpp:84-137) for a 1-channel float image: "Pf\n<w> <h>\n<-1/255 as %lf>\n", rows bottom-up, native
@@ -1593,24 +1564,18 @@ int lexp_save_pfm(const char* path, const float* image, int width, int height, p
 
 int lexp_energy(lexp_ctx* c, int mode, double* data_term, double* smoothness_term) {
     if (!c || mode < 0 || mode > 1 || (!data_term && !smoothness_term)) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_cur_cost[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
-    std::lock_guard<std::mutex> lk(c->mu);
-    c->chain_ok = false;   // copies / other kernels follow on the stream: the next fused launch is an ordinary one
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    LEXP_ENTER(c);
     { int rc = ensure_coef(c, mode); if (rc) return rc; }
     const int H = c->p.height, W = c->p.width;
     const int nblocks = (int)(((size_t)H * W + 255) / 256);
-    double* d_part = nullptr;
-    LEXP_CUDA(cudaMalloc(&d_part, (2 * (size_t)nblocks + 2) * sizeof(double)));
-    LEXP_LAUNCH(lexp_energy_kernel, nblocks, 256, 0, c->stream, c->d_cur_cost[mode], c->d_cur_label[mode], c->d_coef[mode], d_part, H, W, c->sm_lambda, c->sm_th);
-    LEXP_LAUNCH(lexp_energy_finish, 1, 1, 0, c->stream, d_part, nblocks, d_part + 2 * (size_t)nblocks);
-    c->launches += 2;
-    double h[2] = {0.0, 0.0};
-    cudaError_t e = cudaGetLastError();
-    if (e == cudaSuccess) e = cudaMemcpyAsync(h, d_part + 2 * (size_t)nblocks, 2 * sizeof(double), cudaMemcpyDeviceToHost, c->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
-    cudaFree(d_part);
-    if (e != cudaSuccess) return fail(LEXP_ERR_CUDA, std::string("lexp_energy: ") + cudaGetErrorString(e));
+    double h[2] = {0.0, 0.0};   // the two totals, after the 2 * nblocks partial sums in the temporary buffer
+    const int rc = read_back(c, "lexp_energy", (2 * (size_t)nblocks + 2) * sizeof(double), 2 * (size_t)nblocks * sizeof(double), h, sizeof(h), [&](char* d) {
+        double* d_part = reinterpret_cast<double*>(d);
+        cudaError_t e = launch_aux(c, lexp_energy_kernel, nblocks, 256, c->d_cur_cost[mode], c->d_cur_label[mode], c->d_coef[mode], d_part, H, W, c->sm_lambda, c->sm_th);
+        return e == cudaSuccess ? launch_aux(c, lexp_energy_finish, 1, 1, d_part, nblocks, d_part + 2 * (size_t)nblocks) : e;
+    });
+    if (rc) return rc;
     if (data_term) *data_term = h[0];
     if (smoothness_term) *smoothness_term = h[1];
     return LEXP_OK;
@@ -1622,39 +1587,29 @@ int lexp_plan_gc_step(lexp_ctx* c, lexp_plan* pl, int mode, int kind, int m, uin
     if (kind < LEXP_PROP_LIST || kind > LEXP_PROP_RANDOM || m < 0 || m > 120) return fail(LEXP_ERR_INVALID, "bad proposer kind / m");
     if (kind == LEXP_PROP_LIST && !planes) return fail(LEXP_ERR_INVALID, "LEXP_PROP_LIST needs planes");
     if (!pl->d_calls) return fail(LEXP_ERR_STATE, "lexp_plan_set_units has not been called for this plan");
-    if (!c->d_cur_cost[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
-    c->chain_ok = false;   // copies / other kernels around the fused launch: it is an ordinary one
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    LEXP_ENTER(c);
     { int rc = ensure_coef(c, mode); if (rc) return rc; }
+    { int rc = ensure_gc_plan_state(c, pl, mode); if (rc) return rc; }
     const int H = c->p.height, W = c->p.width;
-    if (!c->d_prop_cost[mode]) LEXP_CUDA(cudaMalloc(&c->d_prop_cost[mode], (size_t)H * W * sizeof(float)));
-    if (!pl->d_gc_cells) {
-        int rc = upload_gc_cells(c, pl->ncalls, pl->targ.data(), &pl->d_gc_cells, &pl->gc_nodes);
-        if (rc) return rc;
-        for (const lexp_rect& t : pl->targ) pl->gc_max_nodes = std::max(pl->gc_max_nodes, t.width * t.height);
-    }
     if (pl->gc_nodes > c->gc_scratch_nodes) {   // the residual network of the largest group so far
         LEXP_CUDA(cudaStreamSynchronize(c->stream));
         cudaFree(c->d_gc_scratch); c->d_gc_scratch = nullptr; c->gc_scratch_nodes = 0;
         LEXP_CUDA(cudaMalloc(&c->d_gc_scratch, (size_t)pl->gc_nodes * kGcWords * sizeof(float)));
         c->gc_scratch_nodes = pl->gc_nodes;
     }
-    // (1) the proposals (FastGCStereo.h:47): the PatchMatch phase's device proposers, or the caller's list
+    // (1) the proposals (FastGCStereo.h:47): the caller's list, or the PatchMatch phase's device proposers writing into the plan's
+    // staging buffer
     Plane4* dp = pl->d_planes;
     if (kind == LEXP_PROP_LIST) {
-        if (planes_on_device) dp = const_cast<Plane4*>(reinterpret_cast<const Plane4*>(planes));
-        else LEXP_CUDA(cudaMemcpyAsync(pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4), cudaMemcpyHostToDevice, c->stream));
+        dp = const_cast<Plane4*>(stage_planes(c, pl, planes, planes_on_device));
+        if (!dp) return LEXP_ERR_CUDA;
     }
-    if (kind != LEXP_PROP_LIST || d_planes_out) {
-        LEXP_LAUNCH(lexp_gc_propose_kernel, (pl->ncalls + 127) / 128, 128, 0, c->stream, pl->d_calls, pl->ncalls, dp, reinterpret_cast<Plane4*>(d_planes_out),
-                    (unsigned long long)seed, c->d_cur_label[mode], W, kind, m, c->p.min_disp, c->p.max_disp);
-        LEXP_CUDA(cudaGetLastError());
-        c->launches++;
-    }
+    if (kind != LEXP_PROP_LIST || d_planes_out)
+        LEXP_CUDA(launch_aux(c, lexp_gc_propose_kernel, (pl->ncalls + 127) / 128, 128, pl->d_calls, pl->ncalls, dp, reinterpret_cast<Plane4*>(d_planes_out),
+                             (unsigned long long)seed, c->d_cur_label[mode], W, kind, m, c->p.min_disp, c->p.max_disp));
     // (2) ComputeUnaryPotential(filterRegion, sharedRegion, proposalCost(filterRegion), label) (:49)
     { int rc = run_plan(c, pl, mode, dp, c->d_prop_cost[mode], W, 0, 1); if (rc) return rc; }
-    c->chain_ok = false;
     // (3) expansionMoveBK + copyTo / setTo (:53-59)
     GcParams gp{};
     gp.cells = pl->d_gc_cells; gp.planes = dp; gp.prop_cost = c->d_prop_cost[mode];
@@ -1664,21 +1619,18 @@ int lexp_plan_gc_step(lexp_ctx* c, lexp_plan* pl, int mode, int kind, int m, uin
     gp.H = H; gp.W = W; gp.lambda = c->sm_lambda; gp.th_smooth = c->sm_th;
     gp.relabel_every = c->gc_relabel_every; gp.max_rounds = c->gc_max_rounds;
     if (pl->gc_max_nodes > c->gc_big_nodes) return run_gc_phases(c, pl, gp, d_flows_out);   // large cells: phase kernels over all SMs (blocking)
-    LEXP_LAUNCH(lexp_gc_move_kernel, pl->ncalls, c->gc_threads, 0, c->stream, gp);
-    LEXP_CUDA(cudaGetLastError());
-    c->launches++;
+    LEXP_CUDA(launch_aux(c, lexp_gc_move_kernel, pl->ncalls, c->gc_threads, gp));
     return LEXP_OK;
 }
 
 int lexp_pm_ipc_export(lexp_ctx* c, int mode, void* out) {
     if (!c || !out || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_cur_cost[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
 #ifdef LEXP_EMU
     return fail(LEXP_ERR_INVALID, "no inter-process memory on the emulator");
 #else
     static_assert(sizeof(cudaIpcMemHandle_t) == 64 && LEXP_PM_IPC_BYTES == 3 * 64, "handle layout");
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     cudaIpcMemHandle_t* h = reinterpret_cast<cudaIpcMemHandle_t*>(out);
     LEXP_CUDA(cudaIpcGetMemHandle(&h[0], c->d_cur_cost[mode]));
     LEXP_CUDA(cudaIpcGetMemHandle(&h[1], c->d_cur_label[mode]));
@@ -1689,12 +1641,11 @@ int lexp_pm_ipc_export(lexp_ctx* c, int mode, void* out) {
 
 int lexp_pm_ipc_connect(lexp_ctx* c, int mode, int rank, int world, const void* all) {
     if (!c || !all || mode < 0 || mode > 1 || world < 1 || world > kMaxPeers || rank < 0 || rank >= world) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (!c->d_cur_cost[mode]) return fail(LEXP_ERR_STATE, "lexp_pm_begin has not been called for this view");
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
 #ifdef LEXP_EMU
     return fail(LEXP_ERR_INVALID, "no inter-process memory on the emulator");
 #else
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     lexp_ctx::Peers& pr = c->peers[mode];
     for (int i = 0; i < pr.n_opened; i++) cudaIpcCloseMemHandle(pr.ipc_opened[i]);
     pr = lexp_ctx::Peers();
@@ -1718,8 +1669,7 @@ int lexp_pm_ipc_connect(lexp_ctx* c, int mode, int rank, int world, const void* 
 int lexp_pm_connect_local(lexp_ctx* c, int mode, int rank, int world, lexp_ctx* const* peer_ctx) {
     if (!c || !peer_ctx || mode < 0 || mode > 1 || world < 1 || world > kMaxPeers || rank < 0 || rank >= world) return fail(LEXP_ERR_INVALID, "bad argument");
     if (peer_ctx[rank] != c) return fail(LEXP_ERR_INVALID, "peer_contexts[rank] must be this context");
-    std::lock_guard<std::mutex> lk(c->mu);
-    LEXP_CUDA(cudaSetDevice(c->p.device));
+    LEXP_ENTER(c);
     lexp_ctx::Peers pr;
     int slot = 1;
     for (int r = 0; r < world; r++) {
@@ -1780,6 +1730,18 @@ int sweep_advance(lexp_pm_sweep* s) {
     for (int r = 0; r < kMaxPeers; r++) s->last_rel[r] -= delta;
     s->rel = 0;
     return lexp_pm_advance_epoch(s->ctx, s->mode, delta);
+}
+// The proposal steps of a layer's groups in one iteration: (kind, m) as the `while (prop->isContinued())` loops produce them
+// (FastGCStereo.h:41-46; = localexpstereo_b200.sweep.expand_proposers).  A step's position in the list is its step index.
+std::vector<std::pair<int, int>> expand_proposers(const lexp_pm_sweep* s, int layer, int iteration) {
+    const float range = s->ctx->p.max_disp - s->ctx->p.min_disp;
+    std::vector<std::pair<int, int>> steps;
+    for (auto& pr : s->proposers[layer])
+        for (int it = 0; it < pr.second; it++) {
+            if (pr.first == LEXP_PROP_RANDOM && (double)(range * exp2f(-(float)(iteration + it + 1))) < 0.1) break;   // Proposer.h:149-152
+            steps.push_back({pr.first, pr.first == LEXP_PROP_RANDOM ? iteration + it : 0});
+        }
+    return steps;
 }
 }  // namespace
 
@@ -1879,15 +1841,9 @@ int lexp_pm_sweep_iteration(lexp_pm_sweep* s, int iteration, uint64_t seed, int*
     if (!s || iteration < 0) return fail(LEXP_ERR_INVALID, "bad argument");
     int rc = lexp_pm_reset_sync(s->ctx);
     if (rc) return rc;
-    const float range = s->ctx->p.max_disp - s->ctx->p.min_disp;
     int launches = 0;
     for (auto& g : s->sched) {
-        std::vector<std::pair<int, int>> steps;   // (kind, m) as the `while (prop->isContinued())` loops produce them (FastGCStereo.h:41-46)
-        for (auto& pr : s->proposers[g.layer])
-            for (int it = 0; it < pr.second; it++) {
-                if (pr.first == LEXP_PROP_RANDOM && (double)(range * exp2f(-(float)(iteration + it + 1))) < 0.1) break;   // Proposer.h:149-152
-                steps.push_back({pr.first, pr.first == LEXP_PROP_RANDOM ? iteration + it : 0});
-            }
+        const std::vector<std::pair<int, int>> steps = expand_proposers(s, g.layer, iteration);
         if (steps.empty()) { sweep_group_done(s, {}); continue; }   // every proposer stopped early: no rank launches or publishes anything
         if (g.plan) {
             for (size_t k = 0; k < steps.size(); k++) {
@@ -1908,19 +1864,16 @@ int lexp_pm_sweep_iteration(lexp_pm_sweep* s, int iteration, uint64_t seed, int*
 int lexp_pm_sweep_gc_iteration(lexp_pm_sweep* s, int iteration, uint64_t seed, int* n_steps) {
     if (!s || iteration < 0) return fail(LEXP_ERR_INVALID, "bad argument");
     if (s->world != 1) return fail(LEXP_ERR_INVALID, "the graph-cut iterations run on one GPU (the cell shard covers the PatchMatch phase)");
-    const float range = s->ctx->p.max_disp - s->ctx->p.min_disp;
     int steps_done = 0;
     for (auto& g : s->sched) {
         if (!g.plan) continue;
-        int k = 0;
-        for (auto& pr : s->proposers[g.layer])
-            for (int it = 0; it < pr.second; it++, k++) {
-                if (pr.first == LEXP_PROP_RANDOM && (double)(range * exp2f(-(float)(iteration + it + 1))) < 0.1) break;   // Proposer.h:149-152
-                const int rc = lexp_plan_gc_step(s->ctx, g.plan, s->mode, pr.first, pr.first == LEXP_PROP_RANDOM ? iteration + it : 0,
-                                                 pm_launch_seed(seed, s->mode, iteration, g.layer, g.group, k), nullptr, 0, nullptr, nullptr);
-                if (rc) return rc;
-                steps_done++;
-            }
+        const std::vector<std::pair<int, int>> steps = expand_proposers(s, g.layer, iteration);
+        for (size_t k = 0; k < steps.size(); k++) {
+            const int rc = lexp_plan_gc_step(s->ctx, g.plan, s->mode, steps[k].first, steps[k].second,
+                                             pm_launch_seed(seed, s->mode, iteration, g.layer, g.group, (int)k), nullptr, 0, nullptr, nullptr);
+            if (rc) return rc;
+            steps_done++;
+        }
     }
     if (n_steps) *n_steps = steps_done;
     return LEXP_OK;

@@ -177,24 +177,24 @@ class Plan:
         check(lib().lexp_plan_eval_host_tiles(self.energy._h, self._h, mode, pl.ctypes.data, tiles.ctypes.data, int(with_check)))
         return tiles
 
+    def _planes_ptr(self, planes, planes_on_device):
+        """The planes argument of the C calls: a device pointer as given, or a host copy of num_calls planes kept alive until
+        the next call (the copy out of it is asynchronous)."""
+        if planes_on_device:
+            return int(planes)
+        self._pl_keep = _plane_array(planes)
+        assert len(self._pl_keep) == self.num_calls
+        return self._pl_keep.ctypes.data
+
     def eval_device(self, planes, d_cost_ptr: int, step_bytes: int, with_check=True, mode=0, planes_on_device=False):
         """planes: numpy [n][4] (host) or an int device pointer when planes_on_device."""
-        if planes_on_device:
-            ptr = int(planes)
-        else:
-            self._pl_keep = _plane_array(planes)
-            assert len(self._pl_keep) == self.num_calls
-            ptr = self._pl_keep.ctypes.data
+        ptr = self._planes_ptr(planes, planes_on_device)
         check(lib().lexp_plan_eval_device(self.energy._h, self._h, mode, ptr, int(planes_on_device), int(d_cost_ptr),
                                           int(step_bytes), int(with_check)))
 
     def eval_device_tiles(self, planes, d_tiles_ptr: int, with_check=True, mode=0, planes_on_device=False):
         """Per-call contiguous tiles at d_tiles + sum of previous targetRect areas (floats)."""
-        if planes_on_device:
-            ptr = int(planes)
-        else:
-            self._pl_keep = _plane_array(planes)
-            ptr = self._pl_keep.ctypes.data
+        ptr = self._planes_ptr(planes, planes_on_device)
         check(lib().lexp_plan_eval_device_tiles(self.energy._h, self._h, mode, ptr, int(planes_on_device), int(d_tiles_ptr),
                                                 int(with_check)))
 
@@ -210,14 +210,7 @@ class Plan:
                 publish_epoch=0, wait_epochs=None, wait_mask=0):
         """One proposal step of FastGCStereo.h:41-60 (doGC == false) for all cells of the plan, asynchronous:
         kind = PROP_LIST (planes: numpy [n][4] or a device pointer) | PROP_EXPANSION | PROP_RANDOM (m = outerIter + iter)."""
-        ptr = None
-        if kind == PROP_LIST:
-            if planes_on_device:
-                ptr = int(planes)
-            else:
-                self._pl_keep = _plane_array(planes)
-                assert len(self._pl_keep) == self.num_calls
-                ptr = self._pl_keep.ctypes.data
+        ptr = self._planes_ptr(planes, planes_on_device) if kind == PROP_LIST else None
         we = None
         if wait_mask:
             self._we_keep = np.zeros(8, np.int32)
@@ -228,26 +221,14 @@ class Plan:
 
     def init_step(self, planes, planes_on_device=False, mode=0):
         """initCurrentFast (FastGCStereo.h:101-113) for any energy kind: label and unary cost of every call's targetRect, unconditionally."""
-        if planes_on_device:
-            ptr = int(planes)
-        else:
-            self._pl_keep = _plane_array(planes)
-            assert len(self._pl_keep) == self.num_calls
-            ptr = self._pl_keep.ctypes.data
+        ptr = self._planes_ptr(planes, planes_on_device)
         check(lib().lexp_plan_init_step(self.energy._h, self._h, mode, ptr, int(planes_on_device)))
 
     def gc_step(self, kind, m=0, seed=0, planes=None, planes_on_device=False, d_planes_out=0, d_flows_out=0, mode=0):
         """One proposal step of FastGCStereo.h:41-60 with doGC == true for all cells of the plan, asynchronous: proposal, unary cost,
         FastGCStereo::expansionMoveBK (graph of :424-549 + its minimum cut) and the copyTo / setTo of the winners -- on the device.
         d_flows_out: optional device pointer of double[n] receiving the minimum-cut energy of every move."""
-        ptr = None
-        if kind == PROP_LIST:
-            if planes_on_device:
-                ptr = int(planes)
-            else:
-                self._pl_keep = _plane_array(planes)
-                assert len(self._pl_keep) == self.num_calls
-                ptr = self._pl_keep.ctypes.data
+        ptr = self._planes_ptr(planes, planes_on_device) if kind == PROP_LIST else None
         check(lib().lexp_plan_gc_step(self.energy._h, self._h, mode, int(kind), int(m), int(seed) & 0xFFFFFFFFFFFFFFFF, ptr,
                                       int(planes_on_device), int(d_planes_out) or None, int(d_flows_out) or None))
 

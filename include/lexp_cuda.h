@@ -155,7 +155,9 @@ LEXP_API int lexp_sync(lexp_ctx* ctx);
 /* cudaStream_t of the context (so a caller can order its own device work / events after ours). */
 LEXP_API void* lexp_stream(lexp_ctx* ctx);
 /* Run all subsequent work of this context on the caller's stream (e.g. torch's current stream, or a stream that is
- * being captured into a CUDA graph: lexp_plan_eval_device* issue only graph-capturable work).  Does not synchronise. */
+ * being captured into a CUDA graph).  Does not synchronise.  Under capture, lexp_plan_eval_device*, lexp_plan_pm_step* and the
+ * lexp_pm_sweep iterations issue only graph-capturable work as long as their planes are on the device; a call with host planes
+ * returns LEXP_ERR_INVALID during a capture and enqueues nothing (the capture stays valid). */
 LEXP_API int lexp_set_stream(lexp_ctx* ctx, void* cuda_stream);
 /* Opt in to overlapping launches (programmatic dependent launch) for lexp_plan_eval_device[_tiles] with planes_on_device != 0: a launch
  * may then start -- and read its plane array -- while the context's previous launches are still running (it fills their partly empty
@@ -165,6 +167,9 @@ LEXP_API int lexp_set_stream(lexp_ctx* ctx, void* cuda_stream);
 LEXP_API int lexp_set_overlap(lexp_ctx* ctx, int on);
 /* number of kernels this context has launched so far (bench.py's gpu_launches). */
 LEXP_API int64_t lexp_launch_count(const lexp_ctx* ctx);
+/* how many of this context's launches of lexp_fused_kernel carried the programmatic-serialization attribute, i.e. may have
+ * overlapped the launch before them (0 when the library is built without LEXP_PDL or LEXP_PDL_OFF=1 was set at lexp_create). */
+LEXP_API int64_t lexp_overlapped_launch_count(const lexp_ctx* ctx);
 /* Concurrent lexp_eval_cell calls (the OpenMP loop of FastGCStereo.h:30-49, one blocking call per cell and thread) are
  * combined: calls that arrive while the device is busy are evaluated together in one batched launch.  Returns how many
  * such launches there were and how many calls they served (calls that found the device idle are not counted).

@@ -135,6 +135,7 @@ struct lexp_ctx {
     int gc_big_nodes = 32768;                      // cells with more nodes run as phase kernels over all SMs (LEXP_GC_BIG_NODES)
     int* h_gc_flags = nullptr;                     // pinned: the two decision flags of the phase path
     int64_t launches = 0;
+    int64_t overlapped_launches = 0;   // fused launches that carried the programmatic-serialization attribute
     std::mutex mu;
     int tile_oh = 128;    // max output rows per work item
     bool tile_oh_fixed = false;  // LEXP_TILE_OH given: no per-plan search
@@ -298,6 +299,7 @@ int launch_fused_t(lexp_ctx* c, const KParams& kp_in, int nitems, size_t smem, b
         at[0].val.programmaticStreamSerializationAllowed = 1;
         cfg.attrs = at; cfg.numAttrs = 1;
         LEXP_CUDA(cudaLaunchKernelEx(&cfg, kern, kp));
+        c->overlapped_launches++;
     } else
 #endif
     LEXP_LAUNCH(kern, nitems, kThreads, smem, c->stream, kp);
@@ -514,21 +516,30 @@ int finish_volume(lexp_ctx* c, int mode, int* d_flag) {
     return LEXP_OK;
 }
 
-// The device address of a plan's planes: the caller's device array, or the plan's staging buffer after the host-to-device copy
-// (nullptr: the copy failed)
-const Plane4* stage_planes(lexp_ctx* c, lexp_plan* pl, const lexp_plane* planes, bool on_device) {
-    if (on_device) return reinterpret_cast<const Plane4*>(planes);
+// *out = the device address of a plan's planes: the caller's device array, or the plan's staging buffer after the host-to-device
+// copy.  Host planes are refused while the context's stream is being captured into a CUDA graph: a captured copy would keep the
+// caller's host address, which the Python binding only keeps alive until its next call.  Nothing is enqueued, so the capture stays usable.
+int stage_planes(lexp_ctx* c, lexp_plan* pl, const lexp_plane* planes, bool on_device, const Plane4** out) {
+    *out = reinterpret_cast<const Plane4*>(planes);
+    if (on_device) return LEXP_OK;
+#ifndef LEXP_EMU   // the emulator's streams run synchronously and have no graphs
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    LEXP_CUDA(cudaStreamIsCapturing(c->stream, &cs));
+    if (cs != cudaStreamCaptureStatusNone)
+        return fail(LEXP_ERR_INVALID, "host planes while the context's stream is being captured into a CUDA graph: pass planes on the device");
+#endif
     const cudaError_t e = h2d(c, pl->d_planes, planes, (size_t)pl->ncalls * sizeof(Plane4));
-    if (e != cudaSuccess) { fail(LEXP_ERR_CUDA, std::string("plane upload: ") + cudaGetErrorString(e)); return nullptr; }
-    return pl->d_planes;
+    if (e != cudaSuccess) return fail(LEXP_ERR_CUDA, std::string("plane upload: ") + cudaGetErrorString(e));
+    *out = pl->d_planes;
+    return LEXP_OK;
 }
 
 // lexp_plan_eval_device (row pitch in floats) and lexp_plan_eval_device_tiles (compact tiles)
 int eval_device(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, int planes_on_device, float* d_out, long long pitch,
                 int compact, int with_check) {
     LEXP_ENTER(c);
-    const Plane4* dp = stage_planes(c, pl, planes, planes_on_device);
-    if (!dp) return LEXP_ERR_CUDA;
+    const Plane4* dp = nullptr;
+    { int rc = stage_planes(c, pl, planes, planes_on_device, &dp); if (rc) return rc; }
     return run_plan(c, pl, mode, dp, d_out, pitch, compact, with_check, nullptr, planes_on_device && c->overlap);
 }
 
@@ -537,8 +548,8 @@ int eval_device(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, 
 // and the caller copies it out.
 int eval_host(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, float* d_direct, long long pitch, int compact, int with_check) {
     if (!d_direct) { int rc = ensure_compact(pl, (size_t)pl->sum_s); if (rc) return rc; }
-    const Plane4* dp = stage_planes(c, pl, planes, false);
-    if (!dp) return LEXP_ERR_CUDA;
+    const Plane4* dp = nullptr;
+    { int rc = stage_planes(c, pl, planes, false, &dp); if (rc) return rc; }
     if (!d_direct) return run_plan(c, pl, mode, dp, pl->d_compact, 0, 1, with_check);
     { int rc = run_plan(c, pl, mode, dp, d_direct, pitch, compact, with_check); if (rc) return rc; }
     LEXP_CUDA(cudaStreamSynchronize(c->stream));
@@ -1227,6 +1238,7 @@ int lexp_set_stream(lexp_ctx* c, void* s) {
     return LEXP_OK;
 }
 int64_t lexp_launch_count(const lexp_ctx* c) { return c ? c->launches : 0; }
+int64_t lexp_overlapped_launch_count(const lexp_ctx* c) { return c ? c->overlapped_launches : 0; }
 
 int lexp_set_overlap(lexp_ctx* c, int on) {
     if (!c) return fail(LEXP_ERR_INVALID, "null ctx");
@@ -1331,8 +1343,8 @@ int lexp_plan_pm_step_ex(lexp_ctx* c, lexp_plan* pl, int mode, int step_index, i
     LEXP_ENTER(c);
     const Plane4* dp = nullptr;   // the other kinds: the device proposers generate the planes
     if (kind == LEXP_PROP_LIST) {
-        dp = stage_planes(c, pl, planes, planes_on_device);
-        if (!dp) return LEXP_ERR_CUDA;
+        int rc = stage_planes(c, pl, planes, planes_on_device, &dp);
+        if (rc) return rc;
     }
     PmArgs pm{(flags & LEXP_PM_INIT) ? 2 : 1, kind, m, step_index, (unsigned long long)seed, reinterpret_cast<Plane4*>(d_planes_out),
               publish_epoch, {0, 0, 0, 0, 0, 0, 0, 0}, wait_mask};
@@ -1529,8 +1541,8 @@ int lexp_plan_init_step(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* 
     { int rc = require_pm_state(c, mode); if (rc) return rc; }
     LEXP_ENTER(c);
     { int rc = ensure_gc_plan_state(c, pl, mode); if (rc) return rc; }
-    const Plane4* dp = stage_planes(c, pl, planes, planes_on_device);
-    if (!dp) return LEXP_ERR_CUDA;
+    const Plane4* dp = nullptr;
+    { int rc = stage_planes(c, pl, planes, planes_on_device, &dp); if (rc) return rc; }
     const int W = c->p.width;
     { int rc = run_plan(c, pl, mode, dp, c->d_prop_cost[mode], W, 0, 1); if (rc) return rc; }   // ComputeUnaryPotential (:111)
     LEXP_CUDA(launch_aux(c, lexp_gc_assign_kernel, pl->ncalls, 256, pl->d_gc_cells, dp, c->d_prop_cost[mode], c->d_cur_cost[mode], c->d_cur_label[mode], W));
@@ -1602,8 +1614,10 @@ int lexp_plan_gc_step(lexp_ctx* c, lexp_plan* pl, int mode, int kind, int m, uin
     // staging buffer
     Plane4* dp = pl->d_planes;
     if (kind == LEXP_PROP_LIST) {
-        dp = const_cast<Plane4*>(stage_planes(c, pl, planes, planes_on_device));
-        if (!dp) return LEXP_ERR_CUDA;
+        const Plane4* staged = nullptr;
+        int rc = stage_planes(c, pl, planes, planes_on_device, &staged);
+        if (rc) return rc;
+        dp = const_cast<Plane4*>(staged);
     }
     if (kind != LEXP_PROP_LIST || d_planes_out)
         LEXP_CUDA(launch_aux(c, lexp_gc_propose_kernel, (pl->ncalls + 127) / 128, 128, pl->d_calls, pl->ncalls, dp, reinterpret_cast<Plane4*>(d_planes_out),

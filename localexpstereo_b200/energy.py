@@ -440,6 +440,11 @@ class CostVolumeEnergy:
         return int(lib().lexp_launch_count(self._h))
 
     @property
+    def overlapped_launch_count(self) -> int:
+        """How many of launch_count carried the programmatic-serialization attribute (may have overlapped their predecessor)."""
+        return int(lib().lexp_overlapped_launch_count(self._h))
+
+    @property
     def combine_stats(self):
         """(batched launches that served concurrent single-cell calls, number of calls they served)."""
         b, n = C.c_int64(0), C.c_int64(0)

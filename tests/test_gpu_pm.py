@@ -25,7 +25,7 @@ def devmem():
 
 def run_pm_replay(devmem, H, W, D, windR, units, proposers, iterations=1, seed=1234, scene=None, mode=0):
     import localexpstereo_b200 as L
-    from localexpstereo_b200.sweep import PMSweep, expand_proposers, pm_seed
+    from localexpstereo_b200.sweep import PMSweep, expand_proposers
     imL, imR, volL, volR = scene if scene is not None else make_scene(H, W, D)
     prm = L.Parameters(windR=windR, filterName="GF", filter_param1=1e-4, th_col=0.5)
     E = L.CostVolumeEnergy(imL, imR if mode else None, volL, volR if mode else None, prm, D - 1)
@@ -51,30 +51,39 @@ def run_pm_replay(devmem, H, W, D, windR, units, proposers, iterations=1, seed=1
         # ---- oracle: same initialisation, then the fixed plane sequence step by step
         cost_o = np.full((H, W), np.inf, np.float32)
         lab_o = np.zeros((H, W, 4), np.float32)
-        lay0 = S.lm.layers[0]
         R = windR
         fr0 = [(max(x - R, 0), max(y - R, 0), min(x + w + R, W) - max(x - R, 0), min(y + h + R, H) - max(y - R, 0)) for (x, y, w, h) in S.init_units]
         O.pm_step(Or, S.init_units, S.init_units, fr0, 0, 0, 0, None, cost_o, lab_o, planes=init_labels, init=True, mode=mode)
-        n_prop = n_same = n_close = 0
-        cell_base = np.cumsum([0] + [len(l.unitRegions) for l in S.lm.layers])
-        for it in range(iterations):
-            for g in S.groups:
-                lay = S.lm.layers[g.layer]
-                us = [lay.unitRegions[r] for r in g.cells]; ts = [lay.sharedRegions[r] for r in g.cells]; fs = [lay.filterRegions[r] for r in g.cells]
-                ids = cell_base[g.layer] + g.cells
-                for k, (kind, m) in enumerate(expand_proposers(proposers[g.layer], it, D - 1.0)):
-                    dev_planes = rec_host[(it, g.layer, g.group)][k]
-                    sd = pm_seed(seed, mode, it, g.layer, g.group, k)
-                    for i, u in enumerate(us):   # (1) the oracle's proposer on the oracle's state
-                        mine = O.pm_proposal(kind, m, O.pm_rng_state(sd, ids[i]), lab_o, u, 0.0, D - 1.0)
-                        n_prop += 1
-                        n_same += int(np.array_equal(mine, dev_planes[i]))
-                        n_close += int(np.allclose(mine, dev_planes[i], rtol=2e-6, atol=1e-6))
-                    O.pm_step(Or, us, ts, fs, 0, 0, 0, None, cost_o, lab_o, planes=dev_planes, mode=mode)
-        return dict(cost_d=cost_d, lab_d=lab_d, cost_o=cost_o, lab_o=lab_o, n_prop=n_prop, n_same=n_same, n_close=n_close)
+        r = oracle_pm_replay(Or, S, cost_o, lab_o, rec_host, range(iterations), seed, D)
+        return dict(r, cost_d=cost_d, lab_d=lab_d)
     finally:
         S.close()
         E.close()
+
+
+def oracle_pm_replay(Or, S, cost_o, lab_o, rec_host, iterations, seed, D):
+    """The oracle half of the parity protocol: from the state (cost_o, lab_o), which it updates in place, the oracle runs the pm
+    iterations `iterations` of the PMSweep S with the planes the device recorded, rec_host[(iteration, layer, group)] = [steps][n][4].
+    At every step the oracle's own proposer, run on the oracle's state with the launch's random stream, is compared with the recorded
+    plane.  Returns the oracle's state and the proposal counts that check_pm_result reads."""
+    from localexpstereo_b200.sweep import expand_proposers, pm_seed
+    n_prop = n_same = n_close = 0
+    cell_base = np.cumsum([0] + [len(l.unitRegions) for l in S.lm.layers])
+    for it in iterations:
+        for g in S.groups:
+            lay = S.lm.layers[g.layer]
+            us = [lay.unitRegions[r] for r in g.cells]; ts = [lay.sharedRegions[r] for r in g.cells]; fs = [lay.filterRegions[r] for r in g.cells]
+            ids = cell_base[g.layer] + g.cells
+            for k, (kind, m) in enumerate(expand_proposers(S.proposers[g.layer], it, D - 1.0)):
+                dev_planes = rec_host[(it, g.layer, g.group)][k]
+                sd = pm_seed(seed, S.mode, it, g.layer, g.group, k)
+                for i, u in enumerate(us):   # (1) the oracle's proposer on the oracle's state
+                    mine = O.pm_proposal(kind, m, O.pm_rng_state(sd, ids[i]), lab_o, u, 0.0, D - 1.0)
+                    n_prop += 1
+                    n_same += int(np.array_equal(mine, dev_planes[i]))
+                    n_close += int(np.allclose(mine, dev_planes[i], rtol=2e-6, atol=1e-6))
+                O.pm_step(Or, us, ts, fs, 0, 0, 0, None, cost_o, lab_o, planes=dev_planes, mode=S.mode)
+    return dict(cost_o=cost_o, lab_o=lab_o, n_prop=n_prop, n_same=n_same, n_close=n_close)
 
 
 def check_pm_result(r):

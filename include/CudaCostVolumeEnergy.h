@@ -114,6 +114,10 @@ public:
                               reinterpret_cast<float*>(proposalCost.data), (ptrdiff_t)proposalCost.step, check_valid ? 1 : 0));
     }
 
+    // PMStereoBase::postProcess(currentLabeling_[0], currentLabeling_[1], threshold) (PMStereoBase.h:146-256) on the device state of both
+    // views (PatchMatchPhase for each), in place: the tail of a two-view run (INTEGRATION.md section 4c).  Needs lexp_set_smoothness (omega).
+    void postProcess(float threshold = 1.5f) const { check(lexp_post_process(ctx_, threshold, nullptr)); }
+
     lexp_ctx* context() const { return ctx_; }
     // error state of the per-cell virtuals (they never throw, see guard()): check after the OpenMP region
     bool failed() const { return failed_.load(); }

@@ -284,6 +284,15 @@ LEXP_API int lexp_set_volume_file(lexp_ctx* ctx, int mode, const char* path, int
 LEXP_API int lexp_get_disparities(lexp_ctx* ctx, int mode, float* out_host);
 /* cvutils::io::save_pfm_file (Utilities.hpp:84-137) for a 1-channel float image (disp0.pfm of main.cpp:319,410): byte-identical file. */
 LEXP_API int lexp_save_pfm(const char* path, const float* image, int width, int height, ptrdiff_t step_bytes);
+/* PMStereoBase::postProcess(currentLabeling_[0], currentLabeling_[1], threshold) (PMStereoBase.h:146-256), the last step of a two-view run
+ * (FastGCStereo::run with doDual, :199-217): left-right consistency check with `threshold` (the reference passes 1.5), 3x3 dilation of
+ * the failed pixels, horizontal nearest-neighbour fill and a weighted median over the (2 windR + 1)^2 window (weights exp(-|dI|_1 / omega)
+ * of lexp_set_smoothness), on the device state of BOTH views, which it modifies in place (currentCost_ is not touched).  Equal median
+ * keys, whose order the reference leaves to std::sort, are taken in row-major window order; NaN keys sort last.  `fail_out_host`
+ * (nullable): the two fail maps of the check, uint8[2][H][W] with 0 (consistent), 255 (inconsistent), 128 (matched point outside the
+ * image).  LEXP_ERR_STATE unless lexp_pm_begin has been called for both views and lexp_set_smoothness has set omega.  Read the raw
+ * disparities (disp0raw.pfm) with lexp_get_disparities before this call.  Blocking: returns when the state is final. */
+LEXP_API int lexp_post_process(lexp_ctx* ctx, float threshold, uint8_t* fail_out_host);
 /* Energy of the current state of view `mode`, as the reference logs it (Evaluator / PMStereoBase.h:266): *data_term = sum of currentCost_,
  * *smoothness_term = StereoEnergy::computeSmoothnessCost(currentLabeling_m) (StereoEnergy.h:165-199).  Either pointer may be NULL.  Blocking. */
 LEXP_API int lexp_energy(lexp_ctx* ctx, int mode, double* data_term, double* smoothness_term);

@@ -86,6 +86,7 @@ SYMBOLS = {
     "lexp_set_volume_file": (C.c_int, [_P, C.c_int, C.c_char_p, C.c_int]),
     "lexp_get_disparities": (C.c_int, [_P, C.c_int, _P]),
     "lexp_save_pfm": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.c_ssize_t]),
+    "lexp_post_process": (C.c_int, [_P, C.c_float, _P]),
     "lexp_energy": (C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "lexp_plan_gc_step": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, C.c_int, _P, _P]),
     "lexp_layer_geometry": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), _P, _P, _P, _P]),

@@ -4,6 +4,7 @@
 #include "../../include/lexp_cuda.h"
 #include "lexp_kernels.cuh"
 #include "lexp_gc.cuh"
+#include "lexp_post.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -14,6 +15,7 @@
 #include <chrono>
 #include <thread>
 #include <climits>
+#include <cmath>
 #include <linux/futex.h>
 #include <sys/syscall.h>
 #include <unistd.h>
@@ -126,6 +128,7 @@ struct lexp_ctx {
     } peers[2];
     // pairwise terms / graph-cut move (lexp_gc.cuh; SURVEY.md section 8 f-2, f-3)
     float sm_lambda = 1.0f, sm_omega = 10.0f, sm_th = 1.0f, sm_eps = 0.01f;   // Parameters of main.cpp:73 (paramsGF) / StereoEnergy.h:26-36
+    bool sm_set = false;                           // lexp_set_smoothness has been called (the weighted median of lexp_post_process needs omega)
     float4* d_coef[2] = {nullptr, nullptr};        // forward smoothness coefficients {GE, EG, LG, GG} per pixel (smoothnessCoeff[mode])
     bool coef_valid[2] = {false, false};
     float* d_prop_cost[2] = {nullptr, nullptr};    // proposalCost image of the graph-cut steps (FastGCStereo.h:25)
@@ -134,6 +137,7 @@ struct lexp_ctx {
     int gc_threads = 1024, gc_relabel_every = 24, gc_max_rounds = 1 << 22;
     int gc_big_nodes = 32768;                      // cells with more nodes run as phase kernels over all SMs (LEXP_GC_BIG_NODES)
     int* h_gc_flags = nullptr;                     // pinned: the two decision flags of the phase path
+    char* d_post = nullptr;                        // lexp_post_process scratch: filled labelings, fail maps, row counts / offsets, list, weights
     int64_t launches = 0;
     int64_t overlapped_launches = 0;   // fused launches that carried the programmatic-serialization attribute
     std::mutex mu;
@@ -226,11 +230,15 @@ cudaError_t memset0(lexp_ctx* c, void* dst, size_t bytes) {
     return cudaMemsetAsync(dst, 0, bytes, c->stream);
 }
 template <class... KArgs, class... Args>
-cudaError_t launch_aux(lexp_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, Args... args) {
+cudaError_t launch_aux_smem(lexp_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, Args... args) {
     c->chain_ok = false;
-    LEXP_LAUNCH(kern, grid, block, 0, c->stream, args...);
+    LEXP_LAUNCH(kern, grid, block, smem, c->stream, args...);
     c->launches++;
     return cudaGetLastError();
+}
+template <class... KArgs, class... Args>
+cudaError_t launch_aux(lexp_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, Args... args) {
+    return launch_aux_smem(c, kern, grid, block, 0, args...);
 }
 
 int require_pm_state(const lexp_ctx* c, int mode) {
@@ -670,6 +678,7 @@ int lexp_destroy(lexp_ctx* c) {
         cudaFree(c->d_prop_cost[m]);
     }
     cudaFree(c->d_gc_scratch);
+    cudaFree(c->d_post);
     if (c->h_gc_flags) cudaFreeHost(c->h_gc_flags);
     cudaFree(c->d_sync_arena);
     if (c->own_stream) cudaStreamDestroy(c->stream);
@@ -1491,6 +1500,7 @@ int lexp_set_smoothness(lexp_ctx* c, float lambda, float omega, float th_smooth,
     if (!(omega > 0.0f) || !(lambda >= 0.0f) || !(th_smooth >= 0.0f) || !(epsilon >= 0.0f)) return fail(LEXP_ERR_INVALID, "bad smoothness parameters");
     std::lock_guard<std::mutex> lk(c->mu);
     c->sm_lambda = lambda; c->sm_omega = omega; c->sm_th = th_smooth; c->sm_eps = epsilon;
+    c->sm_set = true;
     c->coef_valid[0] = c->coef_valid[1] = false;
     return LEXP_OK;
 }
@@ -1572,6 +1582,53 @@ int lexp_save_pfm(const char* path, const float* image, int width, int height, p
         ok = fwrite(reinterpret_cast<const char*>(image) + (ptrdiff_t)y * step_bytes, sizeof(float), (size_t)width, f) == (size_t)width;
     ok = (fclose(f) == 0) && ok;
     return ok ? LEXP_OK : fail(LEXP_ERR_INVALID, std::string("write failed: ") + path);
+}
+
+// PMStereoBase::postProcess(currentLabeling_[0], currentLabeling_[1], threshold) (PMStereoBase.h:146-256) on the device state of both
+// views (lexp_post.cuh): five stream-ordered launches, then a synchronise.  windR and omega are the context's, as the reference takes
+// both from one Parameters.  currentCost_ is not touched.
+int lexp_post_process(lexp_ctx* c, float threshold, uint8_t* fail_out_host) {
+    if (!c) return fail(LEXP_ERR_INVALID, "null ctx");
+    for (int m = 0; m < 2; m++) { int rc = require_pm_state(c, m); if (rc) return rc; }
+    LEXP_ENTER(c);
+    if (!c->sm_set) return fail(LEXP_ERR_STATE, "lexp_set_smoothness has not been called: the weighted median needs omega");
+    if (!c->d_guide[0] || !c->d_guide[1]) return fail(LEXP_ERR_STATE, "lexp_set_image has not been called for both views");
+    const int H = c->p.height, W = c->p.width, windR = c->p.windR;
+    const size_t HW = (size_t)H * W;
+    const size_t fill_smem = (size_t)W * sizeof(int);
+    const int nmax = (2 * windR + 1) * (2 * windR + 1);
+    int npow2 = 1;
+    while (npow2 < nmax) npow2 <<= 1;
+    const size_t median_smem = (size_t)npow2 * sizeof(u64) + (size_t)nmax * sizeof(float);
+    if (fill_smem > c->smem_limit || median_smem > c->smem_limit) return fail(LEXP_ERR_INVALID, "post-processing needs more shared memory than the device offers");
+    auto up = [](size_t b) { return (b + 255) / 256 * 256; };
+    const size_t o_list = up(2 * HW * sizeof(float4)), o_fail = o_list + up(2 * HW * sizeof(int)), o_counts = o_fail + up(2 * HW),
+                 o_offsets = o_counts + up(2 * (size_t)H * sizeof(int)), o_wtab = o_offsets + up((2 * (size_t)H + 1) * sizeof(int)),
+                 bytes = o_wtab + up(kPostWeights * sizeof(float));
+    if (!c->d_post) LEXP_CUDA(cudaMalloc(&c->d_post, bytes));
+    float4* d_filled = reinterpret_cast<float4*>(c->d_post);
+    int* d_list = reinterpret_cast<int*>(c->d_post + o_list);
+    unsigned char* d_fail = reinterpret_cast<unsigned char*>(c->d_post + o_fail);
+    int* d_counts = reinterpret_cast<int*>(c->d_post + o_counts);
+    int* d_offsets = reinterpret_cast<int*>(c->d_post + o_offsets);
+    float* d_wtab = reinterpret_cast<float*>(c->d_post + o_wtab);
+    // computePatchWeight (StereoEnergy.h:251-257) for every absdiff: std::exp(float) of the host, as the reference evaluates it
+    float wtab[kPostWeights];
+    for (int k = 0; k < kPostWeights; k++) wtab[k] = std::exp(-(float)k / c->sm_omega);
+    LEXP_CUDA(h2d(c, d_wtab, wtab, sizeof(wtab)));
+    LEXP_CUDA(launch_aux(c, lexp_post_check_kernel, dim3((W + 127) / 128, H, 2), 128, c->d_cur_label[0], c->d_cur_label[1], d_fail, H, W, threshold));
+#ifndef LEXP_EMU
+    LEXP_CUDA(cudaFuncSetAttribute(lexp_post_fill_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)fill_smem));
+    LEXP_CUDA(cudaFuncSetAttribute(lexp_post_median_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)median_smem));
+#endif
+    LEXP_CUDA(launch_aux_smem(c, lexp_post_fill_kernel, dim3(H, 2), kPostThreads, fill_smem, c->d_cur_label[0], c->d_cur_label[1], d_fail, d_filled, d_counts, H, W));
+    LEXP_CUDA(launch_aux(c, lexp_post_offsets_kernel, 1, kPostThreads, d_counts, 2 * H, d_offsets));
+    LEXP_CUDA(launch_aux(c, lexp_post_compact_kernel, dim3(H, 2), kPostThreads, d_fail, d_offsets, d_list, H, W));
+    LEXP_CUDA(launch_aux_smem(c, lexp_post_median_kernel, c->num_sms * kPostMedianCtasPerSm, kPostThreads, median_smem, d_filled, c->d_guide[0], c->d_guide[1],
+                              d_wtab, d_list, d_offsets + 2 * H, c->d_cur_label[0], c->d_cur_label[1], H, W, windR, npow2));
+    if (fail_out_host) LEXP_CUDA(d2h(c, fail_out_host, d_fail, 2 * HW));
+    LEXP_CUDA(cudaStreamSynchronize(c->stream));
+    return LEXP_OK;
 }
 
 int lexp_energy(lexp_ctx* c, int mode, double* data_term, double* smoothness_term) {

@@ -366,6 +366,16 @@ class CostVolumeEnergy:
         check(lib().lexp_get_disparities(self._h, mode, out.ctypes.data))
         return out
 
+    def post_process(self, threshold=1.5, fail_out=None):
+        """PMStereoBase::postProcess(currentLabeling_[0], currentLabeling_[1], threshold) (PMStereoBase.h:146-256) on the device state of
+        both views (pm_begin for each), in place: left-right check, dilation, hole filling, weighted median over windR with the omega of
+        set_smoothness.  `fail_out`: optional uint8 [2][H][W] array that receives the fail maps of the check (0 / 128 / 255).
+        Returns `fail_out`."""
+        if fail_out is not None:
+            assert fail_out.dtype == np.uint8 and fail_out.shape == (2, self.height, self.width) and fail_out.flags.c_contiguous
+        check(lib().lexp_post_process(self._h, float(threshold), None if fail_out is None else fail_out.ctypes.data))
+        return fail_out
+
     def energy(self, mode=0):
         """(data term, smoothness term) of the device state of view `mode`: sum of currentCost_ and
         StereoEnergy::computeSmoothnessCost(currentLabeling_m) (StereoEnergy.h:165-199)."""

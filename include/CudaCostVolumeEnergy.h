@@ -178,9 +178,10 @@ public:
 
     // The PatchMatch phase of FastGCStereo::run on the device: `for (iteration < pmInit) for (layers) localExpansionMovesForLayer_CPU(...,
     // doGC = false)` (FastGCStereo.h:143-157) and initCurrentFast (:94-131), with currentCost_ / currentLabeling_ resident in HBM, the
-    // proposals of ExpansionProposer / RandomProposer drawn on the device and the `cur > prop` update fused into the unary-cost kernel.
+    // proposals of ExpansionProposer / RandomProposer / RansacProposer(1) drawn on the device and the `cur > prop` update fused into the
+    // unary-cost kernel.  graphCutIteration takes the same lists.
     // A maintainer replaces the pm loop of run() by (INTEGRATION.md section 4):
-    //     CudaCostVolumeEnergy::PatchMatchPhase pm(energy, mode, {5, 15, 25}, {{{LEXP_PROP_EXPANSION, 1}, {LEXP_PROP_RANDOM, 8}}, ...});
+    //     CudaCostVolumeEnergy::PatchMatchPhase pm(energy, mode, {5, 15, 25}, {{{LEXP_PROP_EXPANSION, 1}, {LEXP_PROP_RANSAC, 1}, {LEXP_PROP_RANDOM, 7}}, ...});
     //     pm.begin(); pm.init(labels); for (it < pmInit) pm.iteration(it, seed); pm.get(currentCost_[mode], currentLabeling_[mode]);
     class PatchMatchPhase {
         lexp_ctx* ctx_;
@@ -188,7 +189,8 @@ public:
         int mode_;
 
     public:
-        typedef std::vector<std::pair<int, int>> ProposerList;   // (LEXP_PROP_EXPANSION | LEXP_PROP_RANDOM, K) in the order of layer.proposers
+        typedef std::vector<std::pair<int, int>> ProposerList;   // (LEXP_PROP_EXPANSION | LEXP_PROP_RANDOM | LEXP_PROP_RANSAC, K) in the order of
+                                                                 // layer.proposers; LEXP_PROP_RANSAC with K = 1 and world = 1 only
         PatchMatchPhase(const CudaCostVolumeEnergy& e, int mode, const std::vector<int>& unitSizes, const std::vector<ProposerList>& proposers,
                         int rank = 0, int world = 1)
             : ctx_(e.context()), mode_(mode) {

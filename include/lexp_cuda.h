@@ -181,12 +181,17 @@ LEXP_API int lexp_combine_stats(const lexp_ctx* ctx, int64_t* batches, int64_t* 
  *     label = proposer->getNextProposal();  ComputeUnaryPotential(...);  mask = currentCost > proposalCost;
  *     proposalCost.copyTo(currentCost, mask);  currentLabeling.setTo(label, mask);                     (:45-60)
  * with currentCost_[mode] / currentLabeling_[mode] (PMStereoBase.h) resident in HBM, the proposal drawn on the device
- * (ExpansionProposer Proposer.h:69-75, RandomProposer :120-148; cv::RNG-compatible streams, one per cell and step) and the
- * update fused into the epilogue of the unary-cost kernel: nothing crosses PCIe between steps.  The proposal steps of a
- * cell are ordered by per-cell completion counters, so consecutive launches overlap on the device. */
-#define LEXP_PROP_LIST 0       /* planes supplied by the caller (host list replay; the RansacProposer slot) */
+ * (ExpansionProposer Proposer.h:69-75, RandomProposer :120-148, RansacProposer :155-312; cv::RNG-compatible streams, one per cell
+ * and step) and the update fused into the epilogue of the unary-cost kernel: nothing crosses PCIe between steps.  The proposal steps
+ * of a cell are ordered by per-cell completion counters, so consecutive launches overlap on the device.  A LEXP_PROP_RANSAC step is
+ * one launch more: the RANSAC fit of every cell into the plan's plane buffer, ordered after every earlier launch of the stream, which
+ * the step's own launch then reads like a list. */
+#define LEXP_PROP_LIST 0       /* planes supplied by the caller (host list replay) */
 #define LEXP_PROP_EXPANSION 1  /* ExpansionProposer::getNextProposal */
 #define LEXP_PROP_RANDOM 2     /* RandomProposer::getNextProposal, m = outerIter + iter */
+#define LEXP_PROP_RANSAC 3     /* RansacProposer(1)::getNextProposal on the state before the step (DESIGN.md section 3f); m unused.
+                                  Not with LEXP_PM_INIT, and only on one GPU (no multi-GPU cell shard).  The first such step
+                                  of a context allocates an H x W float scratch: issue it before capturing a CUDA graph */
 #define LEXP_PM_INIT 1         /* flags: unconditional write of cost and label (initCurrentFast, FastGCStereo.h:105-113) */
 /* (Re)start the state of view `mode`: currentCost = cost (NULL: +INFINITY, FastGCStereo.h:137), currentLabeling = labeling
  * (NULL: zeros); host arrays float[H][W] / lexp_plane[H][W]. */
@@ -239,8 +244,10 @@ LEXP_API int lexp_pm_advance_epoch(lexp_ctx* ctx, int mode, int delta);
 
 /* ---- The whole PatchMatch phase as one object: what a maintainer calls instead of the pmInit loop of FastGCStereo::run
  * (FastGCStereo.h:143-157).  It owns one plan per (layer, group) of LayerManager::addLayer(unit_sizes[l]) (LayerManager.h:88-185),
- * the proposer list of every layer as (kind, K) pairs in the order of main.cpp:391-397 (LEXP_PROP_EXPANSION / LEXP_PROP_RANDOM; a
- * LEXP_PROP_LIST slot is not allowed here -- use lexp_plan_pm_step for replays), and the epoch bookkeeping of the group boundaries.
+ * the proposer list of every layer as (kind, K) pairs in the order of main.cpp:391-397 (LEXP_PROP_EXPANSION / LEXP_PROP_RANDOM /
+ * LEXP_PROP_RANSAC; a LEXP_PROP_LIST slot is not allowed here -- use lexp_plan_pm_step for replays), and the epoch bookkeeping of the
+ * group boundaries.  LEXP_PROP_RANSAC only with K = 1 (K > 1 would need the snapshot of startIterations to outlive the step) and
+ * world = 1 (the cell shard has no RANSAC support); otherwise LEXP_ERR_INVALID.
  * rank / world: the multi-GPU cell shard (0 / 1 on a single GPU); connect the contexts first (lexp_pm_ipc_connect). */
 typedef struct lexp_pm_sweep lexp_pm_sweep;
 LEXP_API int lexp_pm_sweep_create(lexp_ctx* ctx, int mode, int n_layers, const int* unit_sizes, const int* n_proposers,

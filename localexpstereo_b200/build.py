@@ -8,7 +8,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "liblexp_cuda.so")
 SRCS = [os.path.join(HERE, "csrc", "lexp_capi.cu")]
-DEPS = SRCS + [os.path.join(HERE, "csrc", "lexp_kernels.cuh"), os.path.join(HERE, "csrc", "lexp_gc.cuh"), os.path.join(HERE, "csrc", "lexp_post.cuh"), os.path.join(HERE, "..", "include", "lexp_cuda.h")]
+DEPS = SRCS + [os.path.join(HERE, "csrc", "lexp_kernels.cuh"), os.path.join(HERE, "csrc", "lexp_gc.cuh"), os.path.join(HERE, "csrc", "lexp_post.cuh"), os.path.join(HERE, "csrc", "lexp_ransac.cuh"), os.path.join(HERE, "..", "include", "lexp_cuda.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

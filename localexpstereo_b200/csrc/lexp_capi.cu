@@ -5,6 +5,7 @@
 #include "lexp_kernels.cuh"
 #include "lexp_gc.cuh"
 #include "lexp_post.cuh"
+#include "lexp_ransac.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -138,6 +139,7 @@ struct lexp_ctx {
     int gc_big_nodes = 32768;                      // cells with more nodes run as phase kernels over all SMs (LEXP_GC_BIG_NODES)
     int* h_gc_flags = nullptr;                     // pinned: the two decision flags of the phase path
     char* d_post = nullptr;                        // lexp_post_process scratch: filled labelings, fail maps, row counts / offsets, list, weights
+    float* d_ransac_disp = nullptr;                // LEXP_PROP_RANSAC: float[H][W], the disparities of the snapshot of every cell's unitRegion
     int64_t launches = 0;
     int64_t overlapped_launches = 0;   // fused launches that carried the programmatic-serialization attribute
     std::mutex mu;
@@ -542,6 +544,18 @@ int stage_planes(lexp_ctx* c, lexp_plan* pl, const lexp_plane* planes, bool on_d
     return LEXP_OK;
 }
 
+// LEXP_PROP_RANSAC (lexp_ransac.cuh): the proposal of every cell of the plan into its plane buffer, from the state as the stream has left
+// it.  An ordinary launch (launch_aux clears chain_ok): it starts after every earlier launch has completed, so the snapshot sees all
+// previous steps of the cell, and the launch that reads the planes does not overlap it either.  The cell shard's kernels store into
+// this state from other GPUs and are only ordered by the epoch waits of the fused kernel: refused there.
+int launch_ransac(lexp_ctx* c, lexp_plan* pl, int mode, uint64_t seed) {
+    if (c->peers[mode].world > 1) return fail(LEXP_ERR_INVALID, "LEXP_PROP_RANSAC: the multi-GPU cell shard has no RANSAC support");
+    if (!c->d_ransac_disp) LEXP_CUDA(cudaMalloc(&c->d_ransac_disp, (size_t)c->p.height * c->p.width * sizeof(float)));
+    LEXP_CUDA(launch_aux(c, lexp_ransac_kernel, pl->ncalls, kRansacThreads, pl->d_calls, c->d_cur_label[mode], c->d_ransac_disp, pl->d_planes,
+                         c->p.width, (unsigned long long)seed));
+    return LEXP_OK;
+}
+
 // lexp_plan_eval_device (row pitch in floats) and lexp_plan_eval_device_tiles (compact tiles)
 int eval_device(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* planes, int planes_on_device, float* d_out, long long pitch,
                 int compact, int with_check) {
@@ -679,6 +693,7 @@ int lexp_destroy(lexp_ctx* c) {
     }
     cudaFree(c->d_gc_scratch);
     cudaFree(c->d_post);
+    cudaFree(c->d_ransac_disp);
     if (c->h_gc_flags) cudaFreeHost(c->h_gc_flags);
     cudaFree(c->d_sync_arena);
     if (c->own_stream) cudaStreamDestroy(c->stream);
@@ -1343,8 +1358,9 @@ int lexp_pm_reset_sync(lexp_ctx* c) {
 int lexp_plan_pm_step_ex(lexp_ctx* c, lexp_plan* pl, int mode, int step_index, int kind, int m, uint64_t seed, const lexp_plane* planes,
                          int planes_on_device, lexp_plane* d_planes_out, int flags, int publish_epoch, const int* wait_epochs, unsigned wait_mask) {
     if (!c || !pl || pl->ctx != c || mode < 0 || mode > 1 || step_index < 0) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (kind < LEXP_PROP_LIST || kind > LEXP_PROP_RANDOM || m < 0 || m > 120) return fail(LEXP_ERR_INVALID, "bad proposer kind / m");
+    if (kind < LEXP_PROP_LIST || kind > LEXP_PROP_RANSAC || m < 0 || m > 120) return fail(LEXP_ERR_INVALID, "bad proposer kind / m");
     if (kind == LEXP_PROP_LIST && !planes) return fail(LEXP_ERR_INVALID, "LEXP_PROP_LIST needs planes");
+    if (kind == LEXP_PROP_RANSAC && (flags & LEXP_PM_INIT)) return fail(LEXP_ERR_INVALID, "LEXP_PROP_RANSAC cannot initialise: it fits the current state");
     if (!pl->d_calls || pl->sync_off < 0) return fail(LEXP_ERR_STATE, "lexp_plan_set_units has not been called for this plan");
     { int rc = require_pm_state(c, mode); if (rc) return rc; }
     if (c->p.energy_kind != 0) return fail(LEXP_ERR_INVALID, "the device PatchMatch phase is implemented for the cost-volume energy");
@@ -1354,6 +1370,11 @@ int lexp_plan_pm_step_ex(lexp_ctx* c, lexp_plan* pl, int mode, int step_index, i
     if (kind == LEXP_PROP_LIST) {
         int rc = stage_planes(c, pl, planes, planes_on_device, &dp);
         if (rc) return rc;
+    } else if (kind == LEXP_PROP_RANSAC) {   // the fused launch then reads the plan's plane buffer like a list
+        int rc = launch_ransac(c, pl, mode, seed);
+        if (rc) return rc;
+        dp = pl->d_planes;
+        kind = LEXP_PROP_LIST;
     }
     PmArgs pm{(flags & LEXP_PM_INIT) ? 2 : 1, kind, m, step_index, (unsigned long long)seed, reinterpret_cast<Plane4*>(d_planes_out),
               publish_epoch, {0, 0, 0, 0, 0, 0, 0, 0}, wait_mask};
@@ -1653,7 +1674,7 @@ int lexp_energy(lexp_ctx* c, int mode, double* data_term, double* smoothness_ter
 int lexp_plan_gc_step(lexp_ctx* c, lexp_plan* pl, int mode, int kind, int m, uint64_t seed, const lexp_plane* planes, int planes_on_device,
                       lexp_plane* d_planes_out, double* d_flows_out) {
     if (!c || !pl || pl->ctx != c || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
-    if (kind < LEXP_PROP_LIST || kind > LEXP_PROP_RANDOM || m < 0 || m > 120) return fail(LEXP_ERR_INVALID, "bad proposer kind / m");
+    if (kind < LEXP_PROP_LIST || kind > LEXP_PROP_RANSAC || m < 0 || m > 120) return fail(LEXP_ERR_INVALID, "bad proposer kind / m");
     if (kind == LEXP_PROP_LIST && !planes) return fail(LEXP_ERR_INVALID, "LEXP_PROP_LIST needs planes");
     if (!pl->d_calls) return fail(LEXP_ERR_STATE, "lexp_plan_set_units has not been called for this plan");
     { int rc = require_pm_state(c, mode); if (rc) return rc; }
@@ -1675,6 +1696,10 @@ int lexp_plan_gc_step(lexp_ctx* c, lexp_plan* pl, int mode, int kind, int m, uin
         int rc = stage_planes(c, pl, planes, planes_on_device, &staged);
         if (rc) return rc;
         dp = const_cast<Plane4*>(staged);
+    } else if (kind == LEXP_PROP_RANSAC) {   // then recorded like a list
+        int rc = launch_ransac(c, pl, mode, seed);
+        if (rc) return rc;
+        kind = LEXP_PROP_LIST;
     }
     if (kind != LEXP_PROP_LIST || d_planes_out)
         LEXP_CUDA(launch_aux(c, lexp_gc_propose_kernel, (pl->ncalls + 127) / 128, 128, pl->d_calls, pl->ncalls, dp, reinterpret_cast<Plane4*>(d_planes_out),
@@ -1830,7 +1855,18 @@ int lexp_pm_sweep_create(lexp_ctx* c, int mode, int n_layers, const int* unit_si
     for (int li = 0; li < n_layers; li++) {
         s->proposers.emplace_back();
         for (int j = 0; j < n_prop[li]; j++, pk++) {
-            if ((prop_kind[pk] != LEXP_PROP_EXPANSION && prop_kind[pk] != LEXP_PROP_RANDOM) || prop_K[pk] < 0) { cleanup(); return fail(LEXP_ERR_INVALID, "proposer kinds: LEXP_PROP_EXPANSION / LEXP_PROP_RANDOM"); }
+            if ((prop_kind[pk] != LEXP_PROP_EXPANSION && prop_kind[pk] != LEXP_PROP_RANDOM && prop_kind[pk] != LEXP_PROP_RANSAC) || prop_K[pk] < 0) {
+                cleanup();
+                return fail(LEXP_ERR_INVALID, "proposer kinds: LEXP_PROP_EXPANSION / LEXP_PROP_RANDOM / LEXP_PROP_RANSAC");
+            }
+            if (prop_kind[pk] == LEXP_PROP_RANSAC && prop_K[pk] != 1) {
+                cleanup();
+                return fail(LEXP_ERR_INVALID, "LEXP_PROP_RANSAC with K != 1: later proposals would need the snapshot of startIterations, which is not kept");
+            }
+            if (prop_kind[pk] == LEXP_PROP_RANSAC && world != 1) {
+                cleanup();
+                return fail(LEXP_ERR_INVALID, "LEXP_PROP_RANSAC with world > 1: the multi-GPU cell shard has no RANSAC support");
+            }
             s->proposers.back().push_back({prop_kind[pk], prop_K[pk]});
         }
         int hb = 0, wb = 0;

@@ -140,7 +140,7 @@ def host_unregister(array: np.ndarray):
     check(lib().lexp_host_unregister(array.ctypes.data))
 
 
-PROP_LIST, PROP_EXPANSION, PROP_RANDOM = 0, 1, 2   # LEXP_PROP_* of include/lexp_cuda.h
+PROP_LIST, PROP_EXPANSION, PROP_RANDOM, PROP_RANSAC = 0, 1, 2, 3   # LEXP_PROP_* of include/lexp_cuda.h
 VOL_PLAIN, VOL_FILL, VOL_RIGHT_FROM_LEFT = 0, 1, 2   # LEXP_VOL_*
 
 
@@ -209,7 +209,8 @@ class Plan:
     def pm_step(self, step_index, kind, m=0, seed=0, planes=None, planes_on_device=False, d_planes_out=0, init=False, mode=0,
                 publish_epoch=0, wait_epochs=None, wait_mask=0):
         """One proposal step of FastGCStereo.h:41-60 (doGC == false) for all cells of the plan, asynchronous:
-        kind = PROP_LIST (planes: numpy [n][4] or a device pointer) | PROP_EXPANSION | PROP_RANDOM (m = outerIter + iter)."""
+        kind = PROP_LIST (planes: numpy [n][4] or a device pointer) | PROP_EXPANSION | PROP_RANDOM (m = outerIter + iter) |
+        PROP_RANSAC (RansacProposer(1) on the state before the step; not with init)."""
         ptr = self._planes_ptr(planes, planes_on_device) if kind == PROP_LIST else None
         we = None
         if wait_mask:

@@ -85,13 +85,24 @@ class UnarySweep:
 # PatchMatch phase on the device: FastGCStereo::run's pmInit iterations (FastGCStereo.h:143-157), i.e. the same call
 # schedule with doGC == false, proposals drawn and currentCost_/currentLabeling_ updated on the device (lexp_plan_pm_step).
 # ---------------------------------------------------------------------------------------------------------------------
-from .energy import PROP_EXPANSION, PROP_LIST, PROP_RANDOM  # noqa: E402
+from .energy import PROP_EXPANSION, PROP_LIST, PROP_RANDOM, PROP_RANSAC  # noqa: E402
 
-# the reference's proposer lists (main.cpp:391-397: {Expansion(1), Ransac(1), Random(7)} / {Expansion(2), Ransac(1)} x 2).  The
-# RansacProposer slot (cv::solve SVD + std::random_shuffle on the host) has no device counterpart yet: schedules below give it to
-# the caller (PROP_LIST: planes supplied per step) or, for device-only sweeps, fill it with one more RandomProposer draw so that
-# the number of evaluations per cell stays K = 9 / 3 / 3.
+# The reference's proposer lists (main.cpp:300-306 and 391-397): {Expansion(1), Ransac(1), Random(7)} / {Expansion(2), Ransac(1)} x 2,
+# K = 9 / 3 / 3 evaluations per cell visit.  The RansacProposer runs on the device (PROP_RANSAC, DESIGN.md section 3f).
+V3_PROPOSERS_REFERENCE = [[(PROP_EXPANSION, 1), (PROP_RANSAC, 1), (PROP_RANDOM, 7)], [(PROP_EXPANSION, 2), (PROP_RANSAC, 1)], [(PROP_EXPANSION, 2), (PROP_RANSAC, 1)]]
+# The default schedule of the sweeps and of bench.py: the same K with the RansacProposer slot given to one more RandomProposer draw.
 V3_PROPOSERS_DEVICE = [[(PROP_EXPANSION, 1), (PROP_RANDOM, 8)], [(PROP_EXPANSION, 2), (PROP_RANDOM, 1)], [(PROP_EXPANSION, 2), (PROP_RANDOM, 1)]]
+
+
+def check_ransac_slots(proposers, world):
+    """PROP_RANSAC is supported with K = 1 on one GPU (as lexp_pm_sweep_create checks): RansacProposer::startIterations takes a
+    snapshot that later proposals of the same visit would still fit, and the multi-GPU cell shard has no RANSAC support."""
+    for layer in proposers:
+        for kind, K in layer:
+            if kind == PROP_RANSAC and K != 1:
+                raise ValueError("PROP_RANSAC with K != 1: later proposals would need the snapshot of startIterations, which is not kept")
+            if kind == PROP_RANSAC and world != 1:
+                raise ValueError("PROP_RANSAC with world > 1: the multi-GPU cell shard has no RANSAC support")
 
 
 def pm_seed(base, mode, iteration, layer, group, step):
@@ -173,6 +184,7 @@ class PMSweep:
         self.energy, self.mode, self.rank, self.world = energy, mode, rank, world
         self.unit_sizes = unit_sizes or v3_layer_units(energy.width)
         self.proposers = proposers or V3_PROPOSERS_DEVICE
+        check_ransac_slots(self.proposers, world)
         self.lm = LayerManager(energy.width, energy.height, energy.params.windR)
         self.groups: List[GroupPlan] = []          # this rank's plans
         self.schedule = []                         # every (layer, group) in order: (GroupPlan or None, [ranks that own cells])

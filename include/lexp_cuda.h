@@ -168,7 +168,7 @@ LEXP_API int lexp_set_overlap(lexp_ctx* ctx, int on);
 /* number of kernels this context has launched so far (bench.py's gpu_launches). */
 LEXP_API int64_t lexp_launch_count(const lexp_ctx* ctx);
 /* how many of this context's launches of lexp_fused_kernel carried the programmatic-serialization attribute, i.e. may have
- * overlapped the launch before them (0 when the library is built without LEXP_PDL or LEXP_PDL_OFF=1 was set at lexp_create). */
+ * overlapped the launch before them (0 when LEXP_PDL_OFF=1 was set at lexp_create). */
 LEXP_API int64_t lexp_overlapped_launch_count(const lexp_ctx* ctx);
 /* Concurrent lexp_eval_cell calls (the OpenMP loop of FastGCStereo.h:30-49, one blocking call per cell and thread) are
  * combined: calls that arrive while the device is busy are evaluated together in one batched launch.  Returns how many

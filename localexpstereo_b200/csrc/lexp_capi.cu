@@ -147,7 +147,7 @@ struct lexp_ctx {
     bool tile_oh_fixed = false;  // LEXP_TILE_OH given: no per-plan search
     int num_sms = 132;
     int ctas_per_sm = kMinCtas;  // CTA slots per SM the planner fills (LEXP_CTAS_PER_SM)
-    bool pdl = false;            // launch with programmatic stream serialization (builds with -DLEXP_PDL=1; LEXP_PDL_OFF=1 disables)
+    bool pdl = false;            // launch with programmatic stream serialization (LEXP_PDL_OFF=1 at lexp_create disables)
     bool overlap = false;        // lexp_set_overlap: launches with device-resident planes may overlap their predecessors
     bool chain_ok = false;       // the last operation this context put on its stream was a launch of lexp_fused_kernel: only then may the
                                  // next launch carry the programmatic-serialization attribute.  After a memcpy / memset (plane upload, counter
@@ -300,8 +300,8 @@ int launch_fused_t(lexp_ctx* c, const KParams& kp_in, int nitems, size_t smem, b
         LEXP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_limit));
         c->smem_configured[PM] = true;
     }
-#if LEXP_PDL && !defined(LEXP_EMU)
-    if (c->pdl && allow_pdl && c->chain_ok) {  // programmatic dependent launch: see LEXP_PDL in lexp_kernels.cuh
+#ifndef LEXP_EMU
+    if (c->pdl && allow_pdl && c->chain_ok) {  // programmatic dependent launch: see griddepcontrol in lexp_fused_kernel
         cudaLaunchConfig_t cfg = {};
         cfg.gridDim = dim3((unsigned)nitems); cfg.blockDim = dim3(kThreads); cfg.dynamicSmemBytes = smem; cfg.stream = c->stream;
         cudaLaunchAttribute at[1];
@@ -632,7 +632,7 @@ int lexp_create(const lexp_params* params, lexp_ctx** out_ctx) {
     // kMinCtas CTAs must fit next to each other: 1 KB of every CTA's shared memory is reserved by the system.  With the
     // default build (2 CTAs) no cap is needed: the widest tile needs ~93 KB.
     c->ctas_per_sm = env_int("LEXP_CTAS_PER_SM", kMinCtas);
-    c->pdl = LEXP_PDL && !env_int("LEXP_PDL_OFF", 0);
+    c->pdl = !env_int("LEXP_PDL_OFF", 0);
     c->combine = env_int("LEXP_COMBINE", 1) != 0;
     c->comb_window_us = std::max(0, env_int("LEXP_COMBINE_WINDOW_US", 30));
     c->smem_cap = (size_t)env_int("LEXP_SMEM_CAP", 0);

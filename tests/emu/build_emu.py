@@ -1,19 +1,20 @@
 """TEST INFRASTRUCTURE ONLY.  Builds tests/emu/liblexp_emu.so: the product's own sources (csrc/lexp_capi.cu + lexp_kernels.cuh)
 compiled by g++ with -DLEXP_EMU against tests/emu/cuda_runtime.h, a host emulation of the CUDA execution model (fibers +
 named barriers).  Same C-ABI as liblexp_cuda.so; loaded only by tests/test_emu_*.py, never by the package."""
+import glob
 import os
 import subprocess
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 SRC = os.path.join(ROOT, "localexpstereo_b200", "csrc", "lexp_capi.cu")
-DEPS = [SRC, os.path.join(ROOT, "localexpstereo_b200", "csrc", "lexp_kernels.cuh"), os.path.join(ROOT, "localexpstereo_b200", "csrc", "lexp_gc.cuh"), os.path.join(ROOT, "include", "lexp_cuda.h"),
-        os.path.join(HERE, "cuda_runtime.h"), os.path.abspath(__file__)]
+DEPS = sorted(glob.glob(os.path.join(ROOT, "localexpstereo_b200", "csrc", "*"))) + [
+    os.path.join(ROOT, "include", "lexp_cuda.h"), os.path.join(HERE, "cuda_runtime.h"), os.path.abspath(__file__)]
 SO = os.path.join(HERE, "liblexp_emu.so")
 
 
 def build(force=False, defs=(), tag=""):
-    """`defs`: extra -D flags selecting a build-time kernel variant (e.g. ("-DLEXP_A_ROWTAB=0",)), `tag` names its library."""
+    """`defs`: extra -D flags selecting a build-time kernel variant (e.g. ("-DLEXP_TRACE=1",)), `tag` names its library."""
     so = SO if not tag else os.path.join(HERE, f"liblexp_emu_{tag}.so")
     if os.environ.get("LEXP_EMU_NO_REBUILD") and os.path.exists(so):  # worker processes of a test: the parent has built it
         return so

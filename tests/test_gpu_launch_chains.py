@@ -163,7 +163,7 @@ def devmem():
 
 @pytest.fixture(scope="module")
 def expect_overlap():
-    """The library is built with programmatic dependent launch (LEXP_PDL): the contexts under test must overlap launches."""
+    """The library always launches with programmatic dependent launch unless LEXP_PDL_OFF=1: the contexts under test must overlap launches."""
     return True
 
 

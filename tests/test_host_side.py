@@ -35,6 +35,19 @@ def test_no_cpu_fallback_when_library_is_missing(monkeypatch):
         _capi.lib()
 
 
+def test_every_source_is_a_build_dependency():
+    """An edit to any file lexp_capi.cu includes must rebuild both the product library and the emulator library, or the
+    tests run against the old code."""
+    from localexpstereo_b200 import build
+    from emu import build_emu
+    csrc = os.path.join(ROOT, "localexpstereo_b200", "csrc")
+    sources = [os.path.join(csrc, f) for f in os.listdir(csrc)] + [os.path.join(ROOT, "include", "lexp_cuda.h")]
+    assert len(sources) >= 6
+    for deps in (build.DEPS, build_emu.DEPS):
+        listed = {os.path.realpath(d) for d in deps}
+        assert not [s for s in sources if os.path.realpath(s) not in listed]
+
+
 @pytest.mark.parametrize("W,H,u,windR", [(450, 375, 5, 20), (450, 375, 15, 20), (450, 375, 25, 20), (2048, 1536, 20, 20), (2048, 1536, 61, 20),
                                          (2048, 1536, 184, 20), (1436, 992, 14, 20), (1436, 992, 129, 20), (3840, 2160, 38, 32),
                                          (3840, 2160, 345, 32), (37, 29, 5, 4), (10, 10, 7, 3), (64, 64, 64, 8), (33, 70, 16, 6)])

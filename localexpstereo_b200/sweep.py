@@ -34,6 +34,15 @@ def tile_offsets(target_rects):
     return np.concatenate([[0], np.cumsum(areas)[:-1]]) if len(areas) else np.zeros(0, np.int64), int(areas.sum())
 
 
+def window_rects(units, windR, width, height):
+    """unit +- windR clipped to the image: the filterRegion initCurrentFast gives a unit region (FastGCStereo.h:101-113)."""
+    out = []
+    for (x, y, w, h) in units:
+        x0, y0, x1, y1 = max(x - windR, 0), max(y - windR, 0), min(x + w + windR, width), min(y + h + windR, height)
+        out.append((x0, y0, x1 - x0, y1 - y0))
+    return out
+
+
 @dataclass
 class GroupPlan:
     layer: int
@@ -41,6 +50,18 @@ class GroupPlan:
     cells: np.ndarray        # indices (into the layer's cell list) evaluated by THIS rank
     plan: Plan
     n_steps: int
+    units: list              # unit, target and filter rects of those cells and their global ids, in call order
+    targets: list
+    filters: list
+    ids: np.ndarray
+
+
+def group_plan(energy, lm, li, gi, cells, n_steps=0):
+    """The plan of `cells` of layer li (global cell ids: the cells of the layers before it first, layer after layer)."""
+    lay = lm.layers[li]
+    us, ts, fs = ([rects[r] for r in cells] for rects in (lay.unitRegions, lay.sharedRegions, lay.filterRegions))
+    ids = sum(len(l.unitRegions) for l in lm.layers[:li]) + cells
+    return GroupPlan(li, gi, cells, energy.make_plan(fs, ts), n_steps, us, ts, fs, ids)
 
 
 class UnarySweep:
@@ -65,11 +86,11 @@ class UnarySweep:
                 mine = shard_cells(cells, rank, world)
                 if len(mine) == 0:
                     continue
-                plan = energy.make_plan([lay.filterRegions[r] for r in mine], [lay.sharedRegions[r] for r in mine])
-                self.groups.append(GroupPlan(li, gi, mine, plan, K))
-                self.local_filter_px += K * plan.filter_px
-                self.local_target_px += K * plan.target_px
-                self.local_alg_bytes += K * plan.algorithmic_bytes
+                g = group_plan(energy, self.lm, li, gi, mine, K)
+                self.groups.append(g)
+                self.local_filter_px += K * g.plan.filter_px
+                self.local_target_px += K * g.plan.target_px
+                self.local_alg_bytes += K * g.plan.algorithmic_bytes
         self.launches_per_sweep = sum(g.n_steps for g in self.groups)
 
     def layer(self, li):
@@ -94,11 +115,14 @@ V3_PROPOSERS_REFERENCE = [[(PROP_EXPANSION, 1), (PROP_RANSAC, 1), (PROP_RANDOM, 
 V3_PROPOSERS_DEVICE = [[(PROP_EXPANSION, 1), (PROP_RANDOM, 8)], [(PROP_EXPANSION, 2), (PROP_RANDOM, 1)], [(PROP_EXPANSION, 2), (PROP_RANDOM, 1)]]
 
 
-def check_ransac_slots(proposers, world):
-    """PROP_RANSAC is supported with K = 1 on one GPU (as lexp_pm_sweep_create checks): RansacProposer::startIterations takes a
-    snapshot that later proposals of the same visit would still fit, and the multi-GPU cell shard has no RANSAC support."""
+def check_proposers(proposers, world):
+    """The lists lexp_pm_sweep_create accepts: Expansion, Random and RANSAC slots with K >= 0.  PROP_RANSAC is supported with K = 1
+    on one GPU: RansacProposer::startIterations takes a snapshot that later proposals of the same visit would still fit, and the
+    multi-GPU cell shard has no RANSAC support."""
     for layer in proposers:
         for kind, K in layer:
+            if kind not in (PROP_EXPANSION, PROP_RANDOM, PROP_RANSAC) or K < 0:
+                raise ValueError(f"proposer slot ({kind}, {K}): the sweeps run Expansion, Random and RANSAC slots with K >= 0")
             if kind == PROP_RANSAC and K != 1:
                 raise ValueError("PROP_RANSAC with K != 1: later proposals would need the snapshot of startIterations, which is not kept")
             if kind == PROP_RANSAC and world != 1:
@@ -184,33 +208,28 @@ class PMSweep:
         self.energy, self.mode, self.rank, self.world = energy, mode, rank, world
         self.unit_sizes = unit_sizes or v3_layer_units(energy.width)
         self.proposers = proposers or V3_PROPOSERS_DEVICE
-        check_ransac_slots(self.proposers, world)
+        check_proposers(self.proposers, world)
         self.lm = LayerManager(energy.width, energy.height, energy.params.windR)
         self.groups: List[GroupPlan] = []          # this rank's plans
         self.schedule = []                         # every (layer, group) in order: (GroupPlan or None, [ranks that own cells])
-        sched = pm_schedule(self.lm, self.unit_sizes, world)
-        cell_base = np.cumsum([0] + [len(l.unitRegions) for l in self.lm.layers])   # global cell ids: layer after layer
-        for (li, gi, by_rank, owners) in sched:
-            lay, mine, gp = self.lm.layers[li], by_rank[rank], None
-            if len(mine):
-                plan = energy.make_plan([lay.filterRegions[r] for r in mine], [lay.sharedRegions[r] for r in mine])
-                plan.set_units([lay.unitRegions[r] for r in mine], cell_base[li] + mine)
-                gp = GroupPlan(li, gi, mine, plan, 0)
+        for (li, gi, by_rank, owners) in pm_schedule(self.lm, self.unit_sizes, world):
+            gp = None
+            if len(by_rank[rank]):
+                gp = group_plan(energy, self.lm, li, gi, by_rank[rank])
+                gp.plan.set_units(gp.units, gp.ids)
                 self.groups.append(gp)
             self.schedule.append((li, gi, gp, owners))
         # initCurrentFast (FastGCStereo.h:101-113): every unit region of layer 0 with filterRegion = unit +- windR
-        lay0 = self.lm.layers[0]
-        R, W, H = energy.params.windR, energy.width, energy.height
-        n0 = len(lay0.unitRegions)
+        n0 = len(self.lm.layers[0].unitRegions)
         self.init_owners = [r for r in range(world) if len(range(r, n0, world))]
-        self.init_units = [lay0.unitRegions[r] for r in range(n0)][rank::world]
         self.init_index = np.arange(n0)[rank::world]          # which of the layer-0 units this rank initialises
-        fr = []
-        for (x, y, w, h) in self.init_units:
-            x0, y0, x1, y1 = max(x - R, 0), max(y - R, 0), min(x + w + R, W), min(y + h + R, H)
-            fr.append((x0, y0, x1 - x0, y1 - y0))
-        self.init_plan = energy.make_plan(fr, self.init_units) if len(fr) else None
-        if self.init_plan is not None:
+        self.init_units = [self.lm.layers[0].unitRegions[r] for r in self.init_index]
+        self.init_group = self.init_plan = None       # the initialisation's GroupPlan and its Plan
+        if len(self.init_units):
+            fr = window_rects(self.init_units, energy.params.windR, energy.width, energy.height)
+            self.init_group = GroupPlan(0, 0, self.init_index, energy.make_plan(fr, self.init_units), 0, self.init_units, self.init_units,
+                                        fr, self.init_index)
+            self.init_plan = self.init_group.plan
             self.init_plan.set_units(self.init_units, self.init_index)
         self.clock = EpochClock(rank, world)
 
@@ -228,45 +247,52 @@ class PMSweep:
     def begin(self, cost=None, labeling=None):
         self.energy.pm_begin(self.mode, cost, labeling)
 
+    # ---- the schedule ----------------------------------------------------------------------------------------------------------
+    def group_steps(self, layer, group, iteration, seed):
+        """The proposal steps of one visit of (layer, group) in pm / graph-cut iteration `iteration`: [(index, kind, m, seed)], the
+        seed being the launch's random stream."""
+        E = self.energy
+        return [(k, kind, m, pm_seed(seed, self.mode, iteration, layer, group, k))
+                for k, (kind, m) in enumerate(expand_proposers(self.proposers[layer], iteration, E.MAX_DISPARITY, E.MIN_DISPARITY))]
+
+    def walk(self, iteration, seed, issue):
+        """The PatchMatch-phase walk of the initialisation (iteration None: one PROP_LIST step of init_group) or of one pm iteration.
+        For every group in order it calls issue(group_plan, [(index, kind, m, seed, sync)]) when this rank owns cells of the group,
+        sync being the step's publish_epoch / wait_epochs / wait_mask; then it marks the group done and yields the number of steps
+        issued.  A group whose proposers all stop early publishes nothing on any rank; a rank without cells of a group still counts
+        it.  The launch-chain sync is reset once, before the first group, so all launches of the walk form one chain; the epoch base
+        advances once the walk is exhausted."""
+        self.energy.pm_reset_sync()
+        groups = [(0, 0, self.init_group, self.init_owners)] if iteration is None else self.schedule
+        for (li, gi, g, owners) in groups:
+            steps = [(0, PROP_LIST, 0, 0)] if iteration is None else self.group_steps(li, gi, iteration, seed)
+            if g is not None:
+                issue(g, [(k, kind, m, sd, self.clock.sync_args(k == 0, k == len(steps) - 1)) for (k, kind, m, sd) in steps])
+            self.clock.group_done(owners if steps else [])
+            yield len(steps) if g is not None else 0
+        self._advance()
+
     def init(self, labels):
         """labels [this rank's units of layer 0][4] (all units at world == 1): `currentLabeling(unit) = label;
         ComputeUnaryPotential(unit +- R, unit, ...)` (:107-111)."""
-        self.energy.pm_reset_sync()
-        if self.init_plan is not None:
-            self.init_plan.pm_step(0, PROP_LIST, planes=labels, init=True, mode=self.mode, **self.clock.sync_args(True, True))
-        self.clock.group_done(self.init_owners)
-        self._advance()
+        def issue(g, steps):
+            g.plan.pm_step(0, PROP_LIST, planes=labels, init=True, mode=self.mode, **steps[0][4])
+        for _ in self.walk(None, 0, issue):
+            pass
 
-    def iteration(self, iteration, seed, list_planes=None, planes_out=None):
-        """One pm iteration over all layers (FastGCStereo.h:153-157).  list_planes: {(layer, group): [list steps][n][4]} for PROP_LIST
-        slots; planes_out: optional {(layer, group): device pointer of [steps][n] planes}.  Returns the number of launches."""
-        return sum(self.iteration_by_group(iteration, seed, list_planes, planes_out))
+    def iteration(self, iteration, seed, planes_out=None):
+        """One pm iteration over all layers (FastGCStereo.h:153-157).  planes_out: optional {(layer, group): device pointer of
+        [steps][n] planes}.  Returns the number of launches."""
+        return sum(self.iteration_by_group(iteration, seed, planes_out))
 
-    def iteration_by_group(self, iteration, seed, list_planes=None, planes_out=None):
+    def iteration_by_group(self, iteration, seed, planes_out=None):
         """Generator form of `iteration`: issues one (layer, group) per step and yields its number of launches (lets a
         single-process test interleave several ranks)."""
-        E = self.energy
-        E.pm_reset_sync()
-        for (li, gi, g, owners) in self.schedule:
-            n_launch = 0
-            if g is not None:
-                steps = expand_proposers(self.proposers[li], iteration, E.MAX_DISPARITY, E.MIN_DISPARITY)
-                li_at = 0
-                for k, (kind, m) in enumerate(steps):
-                    pl = None
-                    if kind == PROP_LIST:
-                        pl = list_planes[(li, gi)][li_at]; li_at += 1
-                    out = 0 if planes_out is None else planes_out[(li, gi)] + k * g.plan.num_calls * 16
-                    g.plan.pm_step(k, kind, m, pm_seed(seed, self.mode, iteration, li, gi, k), planes=pl, d_planes_out=out, mode=self.mode,
-                                   **self.clock.sync_args(k == 0, k == len(steps) - 1))
-                    n_launch += 1
-                if not steps:        # every proposer stopped early: nothing is launched for this group on any rank, nothing is published
-                    owners = []
-            elif not expand_proposers(self.proposers[li], iteration, E.MAX_DISPARITY, E.MIN_DISPARITY):
-                owners = []
-            self.clock.group_done(owners)
-            yield n_launch
-        self._advance()
+        def issue(g, steps):
+            for k, kind, m, sd, sync in steps:
+                out = 0 if planes_out is None else planes_out[(g.layer, g.group)] + k * g.plan.num_calls * 16
+                g.plan.pm_step(k, kind, m, sd, d_planes_out=out, mode=self.mode, **sync)
+        return self.walk(iteration, seed, issue)
 
     def get(self, out_cost=None, out_labeling=None):
         return self.energy.pm_get(self.mode, out_cost=out_cost, out_labeling=out_labeling)
@@ -297,23 +323,18 @@ class GCSweep(PMSweep):
         if self.init_plan is not None:
             self.init_plan.init_step(labels, mode=self.mode)
 
-    def gc_iteration(self, iteration, seed, list_planes=None, planes_out=None, flows_out=None, layers=None):
-        """list_planes / planes_out as PMSweep.iteration; flows_out: optional {(layer, group): device pointer of double [steps][n]}
-        receiving the minimum-cut energy of every move; layers: restrict to these layer indices (timing).  Returns the number of
-        proposal steps issued."""
-        E, n = self.energy, 0
+    def gc_iteration(self, iteration, seed, planes_out=None, flows_out=None, layers=None):
+        """planes_out as PMSweep.iteration; flows_out: optional {(layer, group): device pointer of double [steps][n]} receiving the
+        minimum-cut energy of every move; layers: restrict to these layer indices (timing).  Returns the number of proposal steps
+        issued."""
+        n = 0
         for (li, gi, g, _owners) in self.schedule:
             if layers is not None and li not in layers:
                 continue
-            steps = expand_proposers(self.proposers[li], iteration, E.MAX_DISPARITY, E.MIN_DISPARITY)
-            li_at = 0
-            for k, (kind, m) in enumerate(steps):
-                pl = None
-                if kind == PROP_LIST:
-                    pl = list_planes[(li, gi)][li_at]; li_at += 1
+            for k, kind, m, sd in self.group_steps(li, gi, iteration, seed):
                 out = 0 if planes_out is None else planes_out[(li, gi)] + k * g.plan.num_calls * 16
                 fl = 0 if flows_out is None else flows_out[(li, gi)] + k * g.plan.num_calls * 8
-                g.plan.gc_step(kind, m, pm_seed(seed, self.mode, iteration, li, gi, k), planes=pl, d_planes_out=out, d_flows_out=fl, mode=self.mode)
+                g.plan.gc_step(kind, m, sd, d_planes_out=out, d_flows_out=fl, mode=self.mode)
                 n += 1
         return n
 

@@ -5,7 +5,8 @@ import pytest
 from emu import emu_lib
 import test_gpu_zz_gc as _gc
 import test_gpu_zz_gc_phases as _ph
-import test_emu_parity as _ep
+from lexp_replay import SMOOTH, check_gc_result, recording, run_gc_replay
+from lexp_testlib import HostAsDeviceMemory, make_scene
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -23,7 +24,7 @@ def _use_emulator(monkeypatch_module=None):
 
 @pytest.fixture(scope="module")
 def devmem():
-    return _ep._HostAsDeviceMemory()
+    return HostAsDeviceMemory()
 
 
 def test_emu_smoothness_coefficients():
@@ -37,7 +38,7 @@ def test_emu_pairwise_terms():
 def test_emu_gc_replay_small(devmem):
     import localexpstereo_b200 as L   # the GPU test's scene with one graph-cut iteration instead of two (emulation time)
     props = [[(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 2)], [(L.PROP_EXPANSION, 2), (L.PROP_RANDOM, 1)]]
-    _gc.check_gc_result(_gc.run_gc_replay(devmem, 72, 96, 12, 12, [8, 22], props, pm_iterations=1, gc_iterations=1, seed=5))
+    check_gc_result(run_gc_replay(devmem, 72, 96, 12, 12, [8, 22], props, pm_iterations=1, gc_iterations=1, seed=5))
 
 
 def test_emu_gc_replay_right_view_strong_smoothness(devmem):
@@ -63,17 +64,17 @@ def test_emu_gc_result_does_not_depend_on_the_thread_schedule(devmem):
     from localexpstereo_b200.sweep import GCSweep
     from oracle import lexp_oracle as O
     H, W, D, windR = 48, 64, 10, 12
-    imL, _, volL, _ = _gc.make_scene(H, W, D, seed=4)
+    imL, _, volL, _ = make_scene(H, W, D, seed=4)
     props = [[(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 1)]]
     outs = []
     for order in (0, 1, 2):
         with emu_lib.emulated(order=order):
             E = L.CostVolumeEnergy(imL, None, volL, None, L.Parameters(windR=windR, filterName="GF", filter_param1=1e-4, th_col=0.5), D - 1)
-            S = GCSweep(E, unit_sizes=[8], proposers=props, **_gc.SMOOTH)
+            S = GCSweep(E, unit_sizes=[8], proposers=props, **SMOOTH)
             rng = O.CvRNG(3)
             S.begin()
             S.init(np.stack([O.create_random_label(rng, u[0], u[1], 0.0, D - 1.0) for u in S.init_units]))
-            flows = {(g.layer, g.group): devmem.zeros((2, g.plan.num_calls, 2)) for g in S.groups}
+            flows = recording(devmem, S, 0, 21, gc=True)[1]
             S.gc_iteration(0, 21, flows_out={k: devmem.ptr(v) for k, v in flows.items()})
             cost, lab = S.get()
             outs.append((cost, lab, np.concatenate([np.ascontiguousarray(v).view(np.float64).ravel() for v in flows.values()])))

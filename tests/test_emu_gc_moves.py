@@ -7,7 +7,7 @@ import pytest
 
 from emu import emu_lib
 import test_gpu_zz_gc_moves as _mv
-import test_emu_parity as _ep
+from lexp_testlib import HostAsDeviceMemory
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -24,7 +24,7 @@ def _use_emulator():
 
 @pytest.fixture(scope="module")
 def devmem():
-    return _ep._HostAsDeviceMemory()
+    return HostAsDeviceMemory()
 
 
 @pytest.mark.parametrize("mode", [0, 1])

@@ -10,7 +10,7 @@ import pytest
 from emu import emu_lib
 
 import test_gpu_launch_chains as _c
-from test_emu_parity import _HostAsDeviceMemory
+from lexp_testlib import HostAsDeviceMemory
 
 # W not a multiple of 4, generic R; three layers and K = 3 / 2 / 2 steps keep the launch count small
 SCENES = {
@@ -27,7 +27,7 @@ def _use_emulator():
 
 @pytest.fixture(scope="module")
 def devmem():
-    return _HostAsDeviceMemory()
+    return HostAsDeviceMemory()
 
 
 @pytest.fixture(scope="module")

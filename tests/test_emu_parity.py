@@ -9,6 +9,7 @@ suite remains the parity gate for the real device."""
 import pytest
 
 from emu import emu_lib
+from lexp_testlib import HostAsDeviceMemory, make_scene
 
 # the test functions and their fixtures, imported under new names so that pytest collects them here without the gpu mark
 import test_gpu_parity as _p
@@ -24,31 +25,9 @@ def _use_emulator():
 scene = _p.scene
 
 
-class _HostAsDeviceMemory:
-    """On the emulator device memory is host memory: numpy arrays stand in for the device buffers."""
-
-    @staticmethod
-    def zeros(shape, fill=0.0):
-        import numpy as np
-        return np.full(shape, fill, np.float32)
-
-    @staticmethod
-    def upload(a):
-        import numpy as np
-        return np.ascontiguousarray(a)
-
-    @staticmethod
-    def ptr(t):
-        return t.ctypes.data
-
-    @staticmethod
-    def download(t):
-        return t
-
-
 @pytest.fixture(scope="module")
 def devmem():
-    return _HostAsDeviceMemory()
+    return HostAsDeviceMemory()
 
 
 test_emu_device_image_and_tile_outputs = _p.test_device_image_and_tile_outputs
@@ -99,7 +78,7 @@ def test_emu_concurrent_calls_are_combined_into_batched_launches(scene, monkeypa
     from concurrent.futures import ThreadPoolExecutor
     from oracle import lexp_oracle as O
     L, H, W, D = (scene[k] for k in "L H W D".split())
-    imL, imR, volL, volR = _p.make_scene(H, W, D)
+    imL, imR, volL, volR = make_scene(H, W, D)
     prm = L.Parameters(windR=20, filterName="GF", filter_param1=1e-4, th_col=0.5)
     lay = L.LayerManager(W, H, 20).addLayer(7)
     cells = [r for g in lay.disjointRegionSets[:2] for r in g]

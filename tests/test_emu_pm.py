@@ -5,7 +5,7 @@ import pytest
 
 from emu import emu_lib
 import test_gpu_pm as _pm
-import test_emu_parity as _ep
+from lexp_testlib import HostAsDeviceMemory
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -16,7 +16,7 @@ def _use_emulator():
 
 @pytest.fixture(scope="module")
 def devmem():
-    return _ep._HostAsDeviceMemory()
+    return HostAsDeviceMemory()
 
 
 def test_emu_pm_phase_replay_small(devmem):

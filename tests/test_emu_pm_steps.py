@@ -5,7 +5,7 @@ import pytest
 
 from emu import emu_lib
 import test_gpu_zz_pm_steps as _ps
-import test_emu_parity as _ep
+from lexp_testlib import HostAsDeviceMemory
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -16,7 +16,7 @@ def _use_emulator():
 
 @pytest.fixture(scope="module")
 def devmem():
-    return _ep._HostAsDeviceMemory()
+    return HostAsDeviceMemory()
 
 
 @pytest.mark.parametrize("mode", [0, 1])

@@ -4,9 +4,8 @@ small pm and graph-cut iteration with the reference's proposer lists, and the li
 import pytest
 
 from emu import emu_lib
-import test_emu_parity as _ep
 import test_gpu_ransac as _gr
-from lexp_testlib import make_scene
+from lexp_testlib import HostAsDeviceMemory, make_scene
 
 
 @pytest.fixture(scope="module", autouse=True)
@@ -17,7 +16,7 @@ def _use_emulator():
 
 @pytest.fixture(scope="module")
 def devmem():
-    return _ep._HostAsDeviceMemory()
+    return HostAsDeviceMemory()
 
 
 def test_emu_designed_units(devmem):

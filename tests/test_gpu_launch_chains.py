@@ -9,7 +9,6 @@ context under test really overlapped its launches (and the reference did not).
 Scenes: the benchmark's default workload, the R = 16 instantiation (windR 32), a ragged generic-R case (W not a multiple of 4) and
 the NaiveStereoEnergy workload (unary only).  tests/test_emu_launch_chains.py runs the tests without graphs or torch streams on
 the emulator."""
-import contextlib
 import os
 import subprocess
 import sys
@@ -18,7 +17,7 @@ import numpy as np
 import pytest
 
 from oracle import lexp_oracle as O
-from lexp_testlib import assert_costs_close
+from lexp_testlib import TorchDeviceMemory, assert_costs_close, pdl_off
 
 pytestmark = pytest.mark.gpu
 
@@ -37,20 +36,6 @@ SCENES = {
 SMALL = ["ragged_437x291x40_r12", "naive_450x375x64_r20"]
 PM_SCENES = [n for n, s in SCENES.items() if not s.get("naive")]
 PM_SEED = 4321
-
-
-@contextlib.contextmanager
-def pdl_off():
-    """Contexts created inside launch every kernel stream-serialised (lexp_create reads LEXP_PDL_OFF)."""
-    prev = os.environ.get("LEXP_PDL_OFF")
-    os.environ["LEXP_PDL_OFF"] = "1"
-    try:
-        yield
-    finally:
-        if prev is None:
-            os.environ.pop("LEXP_PDL_OFF")
-        else:
-            os.environ["LEXP_PDL_OFF"] = prev
 
 
 class Scene:
@@ -157,8 +142,7 @@ def side_stream():
 
 @pytest.fixture(scope="module")
 def devmem():
-    from test_gpu_parity import _TorchDeviceMemory
-    return _TorchDeviceMemory()
+    return TorchDeviceMemory()
 
 
 @pytest.fixture(scope="module")
@@ -396,12 +380,12 @@ def test_pm_phase_eager_graph_and_native_equal_serialized(pm_scene, side_stream)
 
 def test_pm_replayed_iteration_matches_the_oracle(devmem, side_stream):
     """One captured iteration with planes_out recording, replayed twice: the second replay, re-run by the oracle from the state the
-    first one left (pm_get snapshot) with the planes the device recorded, must satisfy the parity protocol of test_gpu_pm."""
+    first one left (pm_get snapshot) with the planes the device recorded, must satisfy the parity protocol of the PatchMatch replay (tests/lexp_replay.py)."""
     import torch
     import localexpstereo_b200 as L
-    from localexpstereo_b200.sweep import PMSweep, expand_proposers
+    from localexpstereo_b200.sweep import PMSweep
     from lexp_testlib import make_scene
-    from test_gpu_pm import check_pm_result, oracle_pm_replay
+    from lexp_replay import check_pm_result, oracle_replay, pointers, recording
     H, W, D, windR, seed, IT = 120, 170, 16, 20, 9, 1
     props = [[(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 4)], [(L.PROP_EXPANSION, 2), (L.PROP_RANDOM, 1)], [(L.PROP_EXPANSION, 2), (L.PROP_RANDOM, 1)]]
     imL, _, volL, _ = make_scene(H, W, D)
@@ -412,13 +396,13 @@ def test_pm_replayed_iteration_matches_the_oracle(devmem, side_stream):
     try:
         S.begin(); S.init(_pm_labels(S, D)[S.init_index])
         S.iteration(0, seed)
-        rec = {(IT, g.layer, g.group): devmem.zeros((len(expand_proposers(props[g.layer], IT, D - 1.0)), g.plan.num_calls, 4)) for g in S.groups}
+        rec, _ = recording(devmem, S, IT, seed)
         g = torch.cuda.CUDAGraph()
         c0 = E.overlapped_launch_count
         with torch.cuda.stream(side_stream):
             with torch.cuda.graph(g):
                 E.set_stream(torch.cuda.current_stream().cuda_stream)
-                n = S.iteration(IT, seed, planes_out={(l, gr): devmem.ptr(t) for (_, l, gr), t in rec.items()})
+                n = S.iteration(IT, seed, planes_out=pointers(devmem, rec))
             E.set_stream(side_stream.cuda_stream)
             _check_overlapped(E, c0, n, True)
             g.replay()
@@ -430,7 +414,7 @@ def test_pm_replayed_iteration_matches_the_oracle(devmem, side_stream):
         cost_d, lab_d = S.get()
         rec_host = {k: devmem.download(v) for k, v in rec.items()}
         Or = O.CostVolumeEnergyOracle(imL, None, volL, None, windR, 1e-4, 0.5, D - 1)
-        r = oracle_pm_replay(Or, S, cost_s, lab_s, rec_host, [IT], seed, D)
+        r = oracle_replay(Or, S, cost_s, lab_s, [(False, IT, seed)], [rec_host])
         assert not np.array_equal(cost_d, cost_s)   # the replay did move the state
         check_pm_result(dict(r, cost_d=cost_d, lab_d=lab_d))
         del g

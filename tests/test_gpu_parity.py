@@ -3,7 +3,7 @@ import numpy as np
 import pytest
 
 from oracle import lexp_oracle as O
-from lexp_testlib import assert_costs_close, make_scene, random_planes
+from lexp_testlib import TorchDeviceMemory, assert_costs_close, make_scene, random_planes
 
 pytestmark = pytest.mark.gpu
 
@@ -189,36 +189,9 @@ def test_nonzero_min_disparity_and_odd_max(scene):
         E.close()
 
 
-class _TorchDeviceMemory:
-    """Device buffers for the device-output entry points: torch CUDA tensors on the GPU."""
-
-    def __init__(self):
-        import torch
-        self.torch = torch
-
-    # the context launches on its own non-blocking stream: buffers must be complete before their pointers are handed over
-    def zeros(self, shape, fill=0.0):
-        t = self.torch.full(shape, fill, dtype=self.torch.float32, device="cuda")
-        self.torch.cuda.synchronize()
-        return t
-
-    def upload(self, a):
-        t = self.torch.from_numpy(np.ascontiguousarray(a)).cuda()
-        self.torch.cuda.synchronize()
-        return t
-
-    @staticmethod
-    def ptr(t):
-        return t.data_ptr()
-
-    def download(self, t):
-        self.torch.cuda.synchronize()
-        return t.cpu().numpy()
-
-
 @pytest.fixture(scope="module")
 def devmem():
-    return _TorchDeviceMemory()
+    return TorchDeviceMemory()
 
 
 def test_device_image_and_tile_outputs(scene, devmem):

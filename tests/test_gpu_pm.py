@@ -3,104 +3,23 @@ localExpansionMovesForLayer_CPU with doGC == false (FastGCStereo.h:22-72, 94-157
 `mask = cur > prop; copy; setTo` update all on the device (lexp_plan_pm_step), against the numpy oracle (oracle.pm_step, which
 tests/test_ref_pin.py holds bit-identical to the reference's own loop + proposers compiled in oracle/_ref).
 
-Parity protocol (SURVEY.md 8d: "deterministic pm-phase replay"): the device sweep records the plane every (cell, step)
-evaluated; the oracle replays that fixed plane sequence step by step.  Then (1) at every step the oracle's own proposer, run on
+Parity protocol (SURVEY.md 8d: "deterministic pm-phase replay", tests/lexp_replay.py): the device sweep records the plane every
+(cell, step) evaluated; the oracle replays that fixed plane sequence step by step.  Then (1) at every step the oracle's own proposer, run on
 the oracle's state with the same random stream, must produce the plane the device produced; (2) the final costs agree to 1e-4 and
 the final labels are identical except at pixels where the competing costs themselves agree to 1e-4 (the FP32 filter of the device
 vs the reference's double filter can order two nearly equal costs differently)."""
 import numpy as np
 import pytest
 
-from oracle import lexp_oracle as O
-from lexp_testlib import REL_TOL, ABS_FLOOR, make_scene
+from lexp_replay import check_pm_result, run_pm_replay
+from lexp_testlib import TorchDeviceMemory, make_scene
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
 def devmem():
-    from test_gpu_parity import _TorchDeviceMemory
-    return _TorchDeviceMemory()
-
-
-def run_pm_replay(devmem, H, W, D, windR, units, proposers, iterations=1, seed=1234, scene=None, mode=0):
-    import localexpstereo_b200 as L
-    from localexpstereo_b200.sweep import PMSweep, expand_proposers
-    imL, imR, volL, volR = scene if scene is not None else make_scene(H, W, D)
-    prm = L.Parameters(windR=windR, filterName="GF", filter_param1=1e-4, th_col=0.5)
-    E = L.CostVolumeEnergy(imL, imR if mode else None, volL, volR if mode else None, prm, D - 1)
-    Or = O.CostVolumeEnergyOracle(imL, imR if mode else None, volL, volR if mode else None, windR, 1e-4, 0.5, D - 1)
-    S = PMSweep(E, unit_sizes=units, proposers=proposers, mode=mode)
-    try:
-        # ---- device: begin (cost = +inf), initCurrentFast with seeded random labels, `iterations` pm iterations
-        rng = O.CvRNG(seed)
-        init_labels = np.stack([O.create_random_label(rng, u[0] + rng.uniform_int(0, u[2]), u[1] + rng.uniform_int(0, u[3]), 0.0, D - 1.0)
-                                for u in S.init_units])
-        S.begin()
-        S.init(init_labels)
-        rec, rec_host = {}, {}
-        for it in range(iterations):
-            for g in S.groups:
-                nst = len(expand_proposers(proposers[g.layer], it, D - 1.0))
-                rec[(it, g.layer, g.group)] = devmem.zeros((nst, g.plan.num_calls, 4))
-            S.iteration(it, seed, planes_out={(l, gr): devmem.ptr(rec[(it, l, gr)]) for (i2, l, gr) in rec if i2 == it})
-        E.sync()
-        cost_d, lab_d = S.get()
-        for k, v in rec.items():
-            rec_host[k] = devmem.download(v)
-        # ---- oracle: same initialisation, then the fixed plane sequence step by step
-        cost_o = np.full((H, W), np.inf, np.float32)
-        lab_o = np.zeros((H, W, 4), np.float32)
-        R = windR
-        fr0 = [(max(x - R, 0), max(y - R, 0), min(x + w + R, W) - max(x - R, 0), min(y + h + R, H) - max(y - R, 0)) for (x, y, w, h) in S.init_units]
-        O.pm_step(Or, S.init_units, S.init_units, fr0, 0, 0, 0, None, cost_o, lab_o, planes=init_labels, init=True, mode=mode)
-        r = oracle_pm_replay(Or, S, cost_o, lab_o, rec_host, range(iterations), seed, D)
-        return dict(r, cost_d=cost_d, lab_d=lab_d)
-    finally:
-        S.close()
-        E.close()
-
-
-def oracle_pm_replay(Or, S, cost_o, lab_o, rec_host, iterations, seed, D):
-    """The oracle half of the parity protocol: from the state (cost_o, lab_o), which it updates in place, the oracle runs the pm
-    iterations `iterations` of the PMSweep S with the planes the device recorded, rec_host[(iteration, layer, group)] = [steps][n][4].
-    At every step the oracle's own proposer, run on the oracle's state with the launch's random stream, is compared with the recorded
-    plane.  Returns the oracle's state and the proposal counts that check_pm_result reads."""
-    from localexpstereo_b200.sweep import expand_proposers, pm_seed
-    n_prop = n_same = n_close = 0
-    cell_base = np.cumsum([0] + [len(l.unitRegions) for l in S.lm.layers])
-    for it in iterations:
-        for g in S.groups:
-            lay = S.lm.layers[g.layer]
-            us = [lay.unitRegions[r] for r in g.cells]; ts = [lay.sharedRegions[r] for r in g.cells]; fs = [lay.filterRegions[r] for r in g.cells]
-            ids = cell_base[g.layer] + g.cells
-            for k, (kind, m) in enumerate(expand_proposers(S.proposers[g.layer], it, D - 1.0)):
-                dev_planes = rec_host[(it, g.layer, g.group)][k]
-                sd = pm_seed(seed, S.mode, it, g.layer, g.group, k)
-                for i, u in enumerate(us):   # (1) the oracle's proposer on the oracle's state
-                    mine = O.pm_proposal(kind, m, O.pm_rng_state(sd, ids[i]), lab_o, u, 0.0, D - 1.0)
-                    n_prop += 1
-                    n_same += int(np.array_equal(mine, dev_planes[i]))
-                    n_close += int(np.allclose(mine, dev_planes[i], rtol=2e-6, atol=1e-6))
-                O.pm_step(Or, us, ts, fs, 0, 0, 0, None, cost_o, lab_o, planes=dev_planes, mode=S.mode)
-    return dict(cost_o=cost_o, lab_o=lab_o, n_prop=n_prop, n_same=n_same, n_close=n_close)
-
-
-def check_pm_result(r):
-    cd, co, ld, lo = r["cost_d"], r["cost_o"], r["lab_d"], r["lab_o"]
-    assert np.isfinite(co).all() == np.isfinite(cd).all()
-    inv = co == O.COST_FOR_INVALID
-    assert np.array_equal(inv, cd == O.COST_FOR_INVALID)
-    err = np.abs(cd.astype(np.float64) - co) / (REL_TOL * np.maximum(np.abs(co), ABS_FLOOR))
-    assert err[~inv].max() <= 1.0, f"final cost: max err/tol {err[~inv].max():.3f}"
-    diff = (ld != lo).any(axis=2)
-    # a differing label is only acceptable where the two competing costs agree within the tolerance (checked above for the winner:
-    # the costs are within 1e-4 of each other at such pixels) and must be rare
-    assert diff.mean() < 2e-4, f"{diff.sum()} of {diff.size} labels differ"
-    assert r["n_close"] == r["n_prop"], (r["n_close"], r["n_prop"])          # every proposal reproduced (FP64 sin/cos: 1e-6)
-    assert r["n_same"] >= 0.98 * r["n_prop"], (r["n_same"], r["n_prop"])      # and almost all of them bit for bit
-    print(f"pm replay: {r['n_prop']} proposals ({r['n_same']} bit-identical), final cost max err/tol {err[~inv].max():.3f}, "
-          f"{int(diff.sum())} of {diff.size} labels differ")
+    return TorchDeviceMemory()
 
 
 def test_pm_phase_replay_small(devmem):

@@ -12,14 +12,11 @@ import numpy as np
 import pytest
 
 import post_oracle as P
+from lexp_testlib import bits, seeded_labels
 
 pytestmark = pytest.mark.gpu
 
 OMEGA = 10.0
-
-
-def bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
 def make_energy(im0, im1, windR, omega=OMEGA, smooth=True):
@@ -268,14 +265,11 @@ def cones_two_view_state():
     prm = L.Parameters(windR=G["windR"], filterName="GF", filter_param1=1e-4, th_col=0.5)
     E = L.CostVolumeEnergy(G["imL"], G["imR"], G["volL"], G["volR"], prm, G["D"] - 1)
     props = [[(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 2)], [(L.PROP_EXPANSION, 2)], [(L.PROP_EXPANSION, 1)]]
-    from oracle import lexp_oracle as O
     labs = []
     for mode in (0, 1):
         S = GCSweep(E, unit_sizes=[6, 18, 40], proposers=props, mode=mode, lam=1.0, omega=OMEGA, th_smooth=1.0, epsilon=0.01)
-        rng = O.CvRNG(31 + mode)
         S.begin()
-        S.init(np.stack([O.create_random_label(rng, u[0] + rng.uniform_int(0, u[2]), u[1] + rng.uniform_int(0, u[3]), 0.0, G["D"] - 1.0)
-                         for u in S.init_units]))
+        S.init(seeded_labels(S, 31 + mode))
         S.iteration(0, 500 + mode)
         S.gc_iteration(0, 600 + mode)
         labs.append(E.pm_get(mode)[1])

@@ -10,7 +10,8 @@ import numpy as np
 import pytest
 
 from oracle import lexp_oracle as O
-from lexp_testlib import ABS_FLOOR, REL_TOL, make_scene
+from lexp_replay import certify_gc_step
+from lexp_testlib import ABS_FLOOR, REL_TOL, TorchDeviceMemory, energy_and_oracle, make_scene, pdl_off
 import ransac_oracle as RO
 
 pytestmark = pytest.mark.gpu
@@ -18,8 +19,7 @@ pytestmark = pytest.mark.gpu
 
 @pytest.fixture(scope="module")
 def devmem():
-    from test_gpu_parity import _TorchDeviceMemory
-    return _TorchDeviceMemory()
+    return TorchDeviceMemory()
 
 
 def _plane_at(lab, rect, a, b, c):
@@ -84,10 +84,9 @@ def run_ransac_step(devmem, E, lab, units, seed, cell_ids=None, gc=False):
     """One LEXP_PROP_RANSAC step over `units` (one plan, one call per unit, targetRect = unit) from the labeling `lab`; returns the
     recorded planes [n][4]."""
     import localexpstereo_b200 as L
+    from localexpstereo_b200.sweep import window_rects
     H, W = lab.shape[:2]
-    R = E.params.windR
-    fr = [(max(x - R, 0), max(y - R, 0), min(x + w + R, W) - max(x - R, 0), min(y + h + R, H) - max(y - R, 0)) for (x, y, w, h) in units]
-    pl = E.make_plan(fr, units)
+    pl = E.make_plan(window_rects(units, E.params.windR, W, H), units)
     try:
         pl.set_units(units, cell_ids)
         E.pm_begin(0, None, lab)
@@ -180,43 +179,33 @@ class _Recording:
 
 
 # ---- sweeps with the reference's proposer lists ------------------------------------------------------------------------
-def sweep_replay(E, Or, S, iteration, seed, D, gc=False, devmem=None):
+def sweep_replay(E, Or, S, iteration, seed, gc=False, devmem=None):
     """One pm (gc=False) or graph-cut iteration of S issued group by group, with the device's state read back before every RANSAC
     step: each RANSAC proposal must equal the oracle's fit of that state, bit for bit.  Graph-cut: every move of a RANSAC step is
-    certified with test_gpu_zz_gc_moves.certify_gc_step.  pm: the oracle replays the group from the device's state before it, with the
-    planes the device recorded.  Returns (RANSAC proposals checked, labels of the groups' target
-    regions that differ after the replay, labels compared)."""
-    from localexpstereo_b200.sweep import expand_proposers, pm_seed
-    cell_base = np.cumsum([0] + [len(l.unitRegions) for l in S.lm.layers])
-    import test_gpu_zz_gc_moves as _mv
-    n_r = n_diff = n_px = n_moves = 0
-    worst = 0.0
-    E.pm_reset_sync()
-    for (li, gi, g, owners) in S.schedule:
+    certified with certify_gc_step.  pm: the oracle replays the group from the device's state before it, with the planes the device
+    recorded.  Returns (RANSAC proposals checked, labels of the groups' target regions that differ after the replay, labels
+    compared)."""
+    T = dict(n_r=0, n_diff=0, n_px=0, n_moves=0, worst=0.0)
+
+    def issue(g, steps):
         E.sync()
         cost0, lab0 = S.get()
-        steps = expand_proposers(S.proposers[li], iteration, D - 1.0)
         rec = devmem.zeros((len(steps), g.plan.num_calls, 4))
-        lay = S.lm.layers[li]
-        us = [lay.unitRegions[r] for r in g.cells]; ts = [lay.sharedRegions[r] for r in g.cells]; fs = [lay.filterRegions[r] for r in g.cells]
-        ids = cell_base[li] + g.cells
         mine, moved = {}, {}
-        for k, (kind, m) in enumerate(steps):
+        for k, kind, m, sd, sync in steps:
             out = devmem.ptr(rec) + k * g.plan.num_calls * 16
-            sd = pm_seed(seed, S.mode, iteration, li, gi, k)
             if kind == RO.PROP_RANSAC:   # the oracle's fit of the device's state right before the step
                 E.sync()
                 _, lab_pre = S.get()
-                mine[k] = np.stack([RO.ransac_proposal(O.pm_rng_state(sd, ids[i]), lab_pre, u)[0] for i, u in enumerate(us)])
+                mine[k] = np.stack([RO.ransac_proposal(O.pm_rng_state(sd, g.ids[i]), lab_pre, u)[0] for i, u in enumerate(g.units)])
             if gc and kind == RO.PROP_RANSAC:   # every move of the step against the exact minimum cut of the same graph
                 cap = _Recording(devmem)
-                n_moves += len(_mv.certify_gc_step(E, g.plan, ts, S.mode, 1.0, 1.0, cap, kind=kind, m=m, seed=sd, ties_ok=True))
+                T["n_moves"] += len(certify_gc_step(E, g.plan, g.targets, S.mode, 1.0, 1.0, cap, kind=kind, m=m, seed=sd, ties_ok=True))
                 moved[k] = np.array(devmem.download(cap.made[0]))
             elif gc:
                 g.plan.gc_step(kind, m, sd, d_planes_out=out, mode=S.mode)
             else:
-                g.plan.pm_step(k, kind, m, sd, d_planes_out=out, mode=S.mode, **S.clock.sync_args(k == 0, k == len(steps) - 1))
-        S.clock.group_done(owners)
+                g.plan.pm_step(k, kind, m, sd, d_planes_out=out, mode=S.mode, **sync)
         E.sync()
         cost1, lab1 = S.get()
         planes = np.array(devmem.download(rec))
@@ -224,42 +213,36 @@ def sweep_replay(E, Or, S, iteration, seed, D, gc=False, devmem=None):
             planes[k] = pl
         for k, ref in mine.items():
             bad = np.nonzero((planes[k].view(np.uint32) != ref.view(np.uint32)).any(axis=1))[0]
-            assert not len(bad), f"layer {li} group {gi} step {k}: cells {bad[:5]}: device {planes[k][bad[:3]]} oracle {ref[bad[:3]]}"
-            n_r += len(ref)
+            assert not len(bad), f"layer {g.layer} group {g.group} step {k}: cells {bad[:5]}: device {planes[k][bad[:3]]} oracle {ref[bad[:3]]}"
+            T["n_r"] += len(ref)
         if gc:   # the RANSAC moves are certified above; the oracle's FP64 unary costs would not rebuild the device's graphs
-            continue
+            return
         co, lo = cost0.copy(), lab0.copy()
         for k in range(len(steps)):
-            O.pm_step(Or, us, ts, fs, 0, 0, 0, None, co, lo, planes=planes[k], mode=S.mode)
-        for t in ts:
+            O.pm_step(Or, g.units, g.targets, g.filters, 0, 0, 0, None, co, lo, planes=planes[k], mode=S.mode)
+        for t in g.targets:
             sl = (slice(t[1], t[1] + t[3]), slice(t[0], t[0] + t[2]))
-            n_diff += int((lo[sl] != lab1[sl]).any(axis=2).sum())
-            n_px += t[2] * t[3]
+            T["n_diff"] += int((lo[sl] != lab1[sl]).any(axis=2).sum())
+            T["n_px"] += t[2] * t[3]
             # a differing label is only acceptable where the two competing costs agree within the tolerance (RANSAC refits the
             # dominant plane of a cell: its costs are near ties with the current labels, which the FP32 and FP64 filters may order apart)
             inv = co[sl] == O.COST_FOR_INVALID
             assert np.array_equal(inv, cost1[sl] == O.COST_FOR_INVALID)
             err = np.abs(cost1[sl].astype(np.float64) - co[sl]) / (REL_TOL * np.maximum(np.abs(co[sl]), ABS_FLOOR))
-            worst = max(worst, float(err[~inv].max(initial=0.0)))
-    S._advance()
-    assert worst <= 1.0, f"cost max err/tol {worst:.3f}"
-    assert not gc or n_moves == n_r
-    return n_r, n_diff, n_px
+            T["worst"] = max(T["worst"], float(err[~inv].max(initial=0.0)))
+
+    for _ in S.walk(iteration, seed, issue):
+        pass
+    assert T["worst"] <= 1.0, f"cost max err/tol {T['worst']:.3f}"
+    assert not gc or T["n_moves"] == T["n_r"]
+    return T["n_r"], T["n_diff"], T["n_px"]
 
 
 def run_reference_list_iteration(devmem, scene, units, D, windR, seed=5, gc=False, naive=False):
     import localexpstereo_b200 as L
     from localexpstereo_b200 import synth
     from localexpstereo_b200.sweep import GCSweep, PMSweep, V3_PROPOSERS_REFERENCE
-    imL, imR, volL, volR = scene
-    H, W = imL.shape[:2]
-    prm = L.Parameters(windR=windR, filterName="GF", filter_param1=1e-4, th_col=0.5)
-    if naive:
-        E = L.NaiveStereoEnergy(imL, imR, prm, D - 1)
-        Or = O.NaiveStereoEnergyOracle(imL, imR, windR, 1e-4, prm.th_col, prm.th_grad, prm.alpha, D - 1)
-    else:
-        E = L.CostVolumeEnergy(imL, None, volL, None, prm, D - 1)
-        Or = O.CostVolumeEnergyOracle(imL, None, volL, None, windR, 1e-4, 0.5, D - 1)
+    E, Or = energy_and_oracle(scene, D, windR, naive=naive, **(dict(th_col=0.5) if naive else {}))
     S = (GCSweep if gc else PMSweep)(E, unit_sizes=units, proposers=V3_PROPOSERS_REFERENCE)
     try:
         labels = synth.synthetic_planes(S.init_units, 1, D, seed)[0]
@@ -268,7 +251,7 @@ def run_reference_list_iteration(devmem, scene, units, D, windR, seed=5, gc=Fals
         if gc and not naive:   # one pm iteration first, as FastGCStereo::run does before its graph-cut loop (MiddV2 runs none)
             S.iteration(0, seed)
         E.sync()
-        return sweep_replay(E, Or, S, 1 if gc and not naive else 0, seed, D, gc=gc, devmem=devmem)
+        return sweep_replay(E, Or, S, 1 if gc and not naive else 0, seed, gc=gc, devmem=devmem)
     finally:
         S.close()
         E.close()
@@ -325,7 +308,6 @@ def test_reference_lists_launch_chains_equal_serialized(side_stream):
     import localexpstereo_b200 as L
     from localexpstereo_b200 import synth
     from localexpstereo_b200.sweep import PMSweep, V3_PROPOSERS_REFERENCE
-    from test_gpu_launch_chains import pdl_off
     H, W, D, windR = 291, 437, 40, 12
     imL, imR, volL, volR = make_scene(H, W, D)
     prm = L.Parameters(windR=windR, filterName="GF", filter_param1=1e-4, th_col=0.5)
@@ -396,7 +378,6 @@ def test_every_cell_of_sampled_groups_at_2048(devmem):
     try:
         labels = synth.synthetic_planes(S.init_units, 1, D, 7)[0]
         S.begin(); S.init(labels)
-        cell_base = np.cumsum([0] + [len(l.unitRegions) for l in S.lm.layers])
         for when in ("init", "iteration"):
             if when == "iteration":
                 S.iteration(0, 3)
@@ -404,9 +385,7 @@ def test_every_cell_of_sampled_groups_at_2048(devmem):
             cost, lab = S.get()
             for li, gi, every in ((0, 5, 1), (1, 6, 1), (2, 9, 1)):
                 g = next(gp for (l, gr, gp, _) in S.schedule if l == li and gr == gi)
-                cells = g.cells[::every]
-                units = [S.lm.layers[li].unitRegions[r] for r in cells]
-                ids = cell_base[li] + cells
+                units, ids = g.units[::every], g.ids[::every]
                 t0 = time.time()
                 dev = run_ransac_step(devmem, E, lab, units, 11 + li, cell_ids=ids)
                 ref = oracle_planes(lab, units, 11 + li, ids)

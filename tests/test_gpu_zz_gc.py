@@ -7,7 +7,7 @@ iterations of FastGCStereo::run (FastGCStereo.h:22-72 with doGC == true, 411-597
 (oracle.smoothness_coeff, smoothness_terms_expansion, expansion_graph, gc_step) -- which tests/test_ref_pin.py holds against the
 reference's own StereoEnergy and FastGCStereo::expansionMoveBK compiled in oracle/_ref.
 
-Parity protocol of the moves (the same replay as the PatchMatch phase, tests/test_gpu_pm.py): the device sweep records the plane
+Parity protocol of the moves (the same replay as the PatchMatch phase, tests/lexp_replay.py): the device sweep records the plane
 and the minimum-cut energy of every (cell, step); the oracle replays that plane sequence on its own state.  Then (1) the oracle's
 proposer reproduces every device proposal, (2) every move's minimum-cut energy agrees to 1e-5 (the graph the device built from ITS
 unary costs and the cut it found have the value of the oracle's), (3) final costs agree to 1e-4 and final labels are identical
@@ -17,17 +17,15 @@ import numpy as np
 import pytest
 
 from oracle import lexp_oracle as O
-from lexp_testlib import REL_TOL, ABS_FLOOR, make_scene
+from lexp_replay import SMOOTH, check_gc_result, oracle_init, run_gc_replay
+from lexp_testlib import ABS_FLOOR, REL_TOL, TorchDeviceMemory, energy_and_oracle, make_scene, seeded_labels
 
 pytestmark = pytest.mark.gpu
-
-SMOOTH = dict(lam=0.6, omega=10.0, th_smooth=1.0, epsilon=0.01)
 
 
 @pytest.fixture(scope="module")
 def devmem():
-    from test_gpu_parity import _TorchDeviceMemory
-    return _TorchDeviceMemory()
+    return TorchDeviceMemory()
 
 
 def test_smoothness_coefficients_equal_the_oracle():
@@ -77,99 +75,6 @@ def test_pairwise_terms_equal_the_oracle_bit_for_bit():
                         assert np.array_equal(g[t][fi], want[t][k]), (mode, r, t, k, np.abs(g[t][fi] - want[t][k]).max())
     finally:
         E.close()
-
-
-def run_gc_replay(devmem, H, W, D, windR, units, proposers, pm_iterations=1, gc_iterations=1, seed=1234, mode=0, smooth=SMOOTH, scene=None,
-                  naive=False):
-    import localexpstereo_b200 as L
-    from localexpstereo_b200.sweep import GCSweep, expand_proposers, pm_seed
-    imL, imR, volL, volR = scene if scene is not None else make_scene(H, W, D)
-    if naive:   # the image-based energy of `-mode MiddV2` (no cost volume, no device PatchMatch phase: graph-cut iterations only)
-        assert pm_iterations == 0
-        prm = L.Parameters(lambda_=smooth["lam"], windR=windR, filterName="GF", filter_param1=1e-4)
-        E = L.NaiveStereoEnergy(imL, imR, prm, D - 1)
-        Or = O.NaiveStereoEnergyOracle(imL, imR, windR, 1e-4, prm.th_col, prm.th_grad, prm.alpha, D - 1)
-    else:
-        prm = L.Parameters(windR=windR, filterName="GF", filter_param1=1e-4, th_col=0.5)
-        E = L.CostVolumeEnergy(imL, imR if mode else None, volL, volR if mode else None, prm, D - 1)
-        Or = O.CostVolumeEnergyOracle(imL, imR if mode else None, volL, volR if mode else None, windR, 1e-4, 0.5, D - 1)
-    S = GCSweep(E, unit_sizes=units, proposers=proposers, mode=mode, **smooth)
-    coeff = O.smoothness_coeff(imR if mode else imL, smooth["omega"], smooth["epsilon"])
-    lam, th = smooth["lam"], smooth["th_smooth"]
-    try:
-        rng = O.CvRNG(seed)
-        init_labels = np.stack([O.create_random_label(rng, u[0] + rng.uniform_int(0, u[2]), u[1] + rng.uniform_int(0, u[3]), 0.0, D - 1.0)
-                                for u in S.init_units])
-        S.begin()
-        S.init(init_labels)
-        rec, flw = {}, {}
-        for it in range(pm_iterations + gc_iterations):
-            for g in S.groups:
-                nst = len(expand_proposers(proposers[g.layer], it if it < pm_iterations else it - pm_iterations, D - 1.0))
-                rec[(it, g.layer, g.group)] = devmem.zeros((nst, g.plan.num_calls, 4))
-                flw[(it, g.layer, g.group)] = devmem.zeros((nst, g.plan.num_calls, 2))   # one double per (step, cell)
-            po = {(l, gr): devmem.ptr(rec[(i2, l, gr)]) for (i2, l, gr) in rec if i2 == it}
-            if it < pm_iterations:
-                S.iteration(it, seed, planes_out=po)
-            else:   # both loops of FastGCStereo::run restart `iteration` at 0 (FastGCStereo.h:143,171)
-                S.gc_iteration(it - pm_iterations, seed + 1, planes_out=po, flows_out={(l, gr): devmem.ptr(flw[(i2, l, gr)]) for (i2, l, gr) in flw if i2 == it})
-        E.sync()
-        cost_d, lab_d = S.get()
-        rec_host = {k: devmem.download(v) for k, v in rec.items()}
-        flw_host = {k: np.ascontiguousarray(devmem.download(v)).view(np.float64)[..., 0] for k, v in flw.items()}
-        # ---- oracle replay
-        cost_o = np.full((H, W), np.inf, np.float32)
-        lab_o = np.zeros((H, W, 4), np.float32)
-        R = windR
-        fr0 = [(max(x - R, 0), max(y - R, 0), min(x + w + R, W) - max(x - R, 0), min(y + h + R, H) - max(y - R, 0)) for (x, y, w, h) in S.init_units]
-        O.pm_step(Or, S.init_units, S.init_units, fr0, 0, 0, 0, None, cost_o, lab_o, planes=init_labels, init=True, mode=mode)
-        n_prop = n_close = n_moves = 0
-        worst_flow = 0.0
-        cell_base = np.cumsum([0] + [len(l.unitRegions) for l in S.lm.layers])
-        for it in range(pm_iterations + gc_iterations):
-            gc, oit = it >= pm_iterations, (it if it < pm_iterations else it - pm_iterations)
-            for g in S.groups:
-                lay = S.lm.layers[g.layer]
-                us = [lay.unitRegions[r] for r in g.cells]; ts = [lay.sharedRegions[r] for r in g.cells]; fs = [lay.filterRegions[r] for r in g.cells]
-                ids = cell_base[g.layer] + g.cells
-                for k, (kind, m) in enumerate(expand_proposers(proposers[g.layer], oit, D - 1.0)):
-                    dev_planes = rec_host[(it, g.layer, g.group)][k]
-                    sd = pm_seed(seed + (1 if gc else 0), mode, oit, g.layer, g.group, k)
-                    for i, u in enumerate(us):
-                        mine = O.pm_proposal(kind, m, O.pm_rng_state(sd, ids[i]), lab_o, u, 0.0, D - 1.0)
-                        n_prop += 1
-                        n_close += int(np.allclose(mine, dev_planes[i], rtol=2e-6, atol=1e-6))
-                    if not gc:
-                        O.pm_step(Or, us, ts, fs, 0, 0, 0, None, cost_o, lab_o, planes=dev_planes, mode=mode)
-                    else:
-                        _, flows = O.gc_step(Or, us, ts, fs, 0, 0, 0, None, cost_o, lab_o, coeff, lam, th, planes=dev_planes, mode=mode)
-                        df = flw_host[(it, g.layer, g.group)][k]
-                        worst_flow = max(worst_flow, float((np.abs(df - flows) / np.maximum(np.abs(flows), 1e-3)).max()))
-                        n_moves += len(us)
-        e_d = float(cost_d.astype(np.float64).sum()) + O.smoothness_cost(lab_d, coeff, lam, th)
-        e_o = float(cost_o.astype(np.float64).sum()) + O.smoothness_cost(lab_o, coeff, lam, th)
-        return dict(cost_d=cost_d, lab_d=lab_d, cost_o=cost_o, lab_o=lab_o, n_prop=n_prop, n_close=n_close, n_moves=n_moves, worst_flow=worst_flow,
-                    e_d=e_d, e_o=e_o)
-    finally:
-        S.close()
-        E.close()
-
-
-def check_gc_result(r, max_label_fraction=2e-3):
-    cd, co, ld, lo = r["cost_d"], r["cost_o"], r["lab_d"], r["lab_o"]
-    diff = (ld != lo).any(axis=2)
-    same = ~diff
-    inv = co == O.COST_FOR_INVALID
-    assert np.array_equal(inv[same], (cd == O.COST_FOR_INVALID)[same])
-    err = np.abs(cd.astype(np.float64) - co) / (REL_TOL * np.maximum(np.abs(co), ABS_FLOOR))
-    sel = same & ~inv
-    assert err[sel].max() <= 1.0, f"final cost: max err/tol {err[sel].max():.3f}"
-    assert r["n_moves"] > 0 and r["worst_flow"] <= 1e-5, f"minimum-cut energy of a move: rel err {r['worst_flow']:.2e}"
-    assert diff.mean() <= max_label_fraction, f"{diff.sum()} of {diff.size} labels differ"
-    assert abs(r["e_d"] - r["e_o"]) <= 1e-5 * abs(r["e_o"]), (r["e_d"], r["e_o"])
-    assert r["n_close"] >= r["n_prop"] - 2 * int(diff.sum()), (r["n_close"], r["n_prop"])   # a differing label can be drawn as a proposal source
-    print(f"gc replay: {r['n_moves']} moves, min-cut energy max rel err {r['worst_flow']:.1e}, final cost max err/tol {err[sel].max():.3f}, "
-          f"{int(diff.sum())} of {diff.size} labels differ, energy {r['e_d']:.6f} vs {r['e_o']:.6f}")
 
 
 def test_gc_replay_small(devmem):
@@ -251,58 +156,49 @@ def test_gc_iteration_on_the_image_based_energy(devmem):
     to 1e-5, costs wherever the labels agree, labels up to those ties."""
     import lexp_golden
     import localexpstereo_b200 as L
-    from localexpstereo_b200.sweep import GCSweep, expand_proposers, pm_seed
+    from localexpstereo_b200.sweep import GCSweep
     G = lexp_golden.load()
     imL, imR = G["imL"], G["imR"]
     H, W = imL.shape[:2]
     D, windR = 64, 20
     lam, omega, th, eps = 20.0, 10.0, 1.0, 0.01
-    prm = L.Parameters(lambda_=lam, windR=windR, filterName="GF", filter_param1=1e-4)
-    E = L.NaiveStereoEnergy(imL, imR, prm, D - 1)
-    Or = O.NaiveStereoEnergyOracle(imL, imR, windR, 1e-4, prm.th_col, prm.th_grad, prm.alpha, D - 1)
+    E, Or = energy_and_oracle((imL, imR, None, None), D, windR, naive=True, lambda_=lam)
     props = [[(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 1)], [(L.PROP_EXPANSION, 1)]]
     S = GCSweep(E, unit_sizes=[5, 15], proposers=props, lam=lam, omega=omega, th_smooth=th, epsilon=eps)
     coeff = O.smoothness_coeff(imL, omega, eps)
     try:
-        rng = O.CvRNG(8)
-        labels = np.stack([O.create_random_label(rng, u[0] + rng.uniform_int(0, u[2]), u[1] + rng.uniform_int(0, u[3]), 0.0, D - 1.0) for u in S.init_units])
+        labels = seeded_labels(S, 8)
         S.begin()
         S.init(labels)
         cost_d, lab_d = S.get()
-        cost_o, lab_o = np.full((H, W), np.inf, np.float32), np.zeros((H, W, 4), np.float32)
-        R = windR
-        fr0 = [(max(x - R, 0), max(y - R, 0), min(x + w + R, W) - max(x - R, 0), min(y + h + R, H) - max(y - R, 0)) for (x, y, w, h) in S.init_units]
-        O.pm_step(Or, S.init_units, S.init_units, fr0, 0, 0, 0, None, cost_o, lab_o, planes=labels, init=True)
+        cost_o, lab_o = oracle_init(Or, S, labels)
         assert np.array_equal(lab_d, lab_o) and np.array_equal(cost_d == O.COST_FOR_INVALID, cost_o == O.COST_FOR_INVALID)
         ok = cost_o != O.COST_FOR_INVALID
         assert (np.abs(cost_d[ok] - cost_o[ok]) <= REL_TOL * np.maximum(np.abs(cost_o[ok]), ABS_FLOOR)).all()
         n_moves = n_diff = 0
         worst_flow = worst_cost = 0.0
-        cell_base = np.cumsum([0] + [len(l.unitRegions) for l in S.lm.layers])
         for g in S.groups:
             if g.group not in (0, 5, len(S.lm.layers[g.layer].disjointRegionSets) - 1):   # three groups per layer (emulation time)
                 continue
-            lay = S.lm.layers[g.layer]
-            us = [lay.unitRegions[r] for r in g.cells]; ts = [lay.sharedRegions[r] for r in g.cells]; fs = [lay.filterRegions[r] for r in g.cells]
-            for k, (kind, m) in enumerate(expand_proposers(props[g.layer], 0, D - 1.0)):
+            for k, kind, m, sd in S.group_steps(g.layer, g.group, 0, 3):
                 pre_c, pre_l = S.get()
                 rec, flw = devmem.zeros((g.plan.num_calls, 4)), devmem.zeros((g.plan.num_calls, 2))
-                g.plan.gc_step(kind, m, pm_seed(3, 0, 0, g.layer, g.group, k), d_planes_out=devmem.ptr(rec), d_flows_out=devmem.ptr(flw))
+                g.plan.gc_step(kind, m, sd, d_planes_out=devmem.ptr(rec), d_flows_out=devmem.ptr(flw))
                 E.sync()
                 post_c, post_l = S.get()
                 dev_planes = devmem.download(rec)
                 flows_d = np.ascontiguousarray(devmem.download(flw)).view(np.float64)[:, 0]
-                for i, u in enumerate(us):   # the device's proposer against the oracle's, on the same state
-                    mine = O.pm_proposal(kind, m, O.pm_rng_state(pm_seed(3, 0, 0, g.layer, g.group, k), cell_base[g.layer] + g.cells[i]), pre_l, u, 0.0, D - 1.0)
+                for i, u in enumerate(g.units):   # the device's proposer against the oracle's, on the same state
+                    mine = O.pm_proposal(kind, m, O.pm_rng_state(sd, g.ids[i]), pre_l, u, 0.0, D - 1.0)
                     assert np.allclose(mine, dev_planes[i], rtol=2e-6, atol=1e-6)
                 oc, ol = pre_c.copy(), pre_l.copy()
-                _, flows_o = O.gc_step(Or, us, ts, fs, 0, 0, 0, None, oc, ol, coeff, lam, th, planes=dev_planes)
+                _, flows_o = O.gc_step(Or, g.units, g.targets, g.filters, 0, 0, 0, None, oc, ol, coeff, lam, th, planes=dev_planes)
                 worst_flow = max(worst_flow, float((np.abs(flows_d - flows_o) / np.maximum(np.abs(flows_o), 1e-3)).max()))
                 diff = (post_l != ol).any(axis=2)
                 same = ~diff & (oc != O.COST_FOR_INVALID)
                 assert np.array_equal((post_c == O.COST_FOR_INVALID)[~diff], (oc == O.COST_FOR_INVALID)[~diff])
                 worst_cost = max(worst_cost, float((np.abs(post_c[same].astype(np.float64) - oc[same]) / (REL_TOL * np.maximum(np.abs(oc[same]), ABS_FLOOR))).max()))
-                n_diff += int(diff.sum()); n_moves += len(us)
+                n_diff += int(diff.sum()); n_moves += len(g.units)
         print(f"naive gc: {n_moves} moves, min-cut energy max rel err {worst_flow:.1e}, cost max err/tol {worst_cost:.3f}, {n_diff} label ties")
         assert n_moves > 300 and worst_flow <= 1e-5 and worst_cost <= 1.0, (n_moves, worst_flow, worst_cost)
         assert n_diff <= 2e-2 * H * W, n_diff

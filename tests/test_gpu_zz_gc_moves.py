@@ -3,7 +3,7 @@
 The oracle gets the device's own inputs: the pre-move state (pm_get), the device's coefficient maps (smooth_coeff) and the device's proposal
 costs (the plan's own unary launch with image output and the validity check, which is what lexp_plan_gc_step writes into its internal
 image).  oracle.expansion_graph then builds the graph lexp_gc.cuh builds, bit for bit (same add_tweights order, bit-identical pair terms),
-and only the solver is left to compare.  Per move (certify_gc_step):
+and only the solver is left to compare.  Per move (lexp_replay.certify_gc_step):
   (a) every pixel of a cell holds its pre-move (cost, label) or (proposal cost, proposal), bit for bit; nothing outside the cells changes;
   (b) duality: the device's flow minus BK's constant `konst` equals the value of the device's own cut; a flow and a cut of equal value are
       both optimal, whatever the oracle's solver does;
@@ -22,47 +22,21 @@ import math
 import numpy as np
 import pytest
 
-from oracle import c_oracle
 from oracle import lexp_oracle as O
+from lexp_replay import REPORT, U, certify_gc_step, proposal_costs
+from lexp_testlib import TorchDeviceMemory, bits, seeded_labels
 
 pytestmark = pytest.mark.gpu
 
 INVALID = O.COST_FOR_INVALID
-U = 2.0 ** -53
-ARCS = ((1, 0), (0, 1), (-1, 1), (1, 1))      # the forward arcs GE, EG, LG, GG: cap[0..3] of oracle.expansion_graph
 FAR = np.array([0, 0, -4, 0], np.float32)     # disparity -4 < MIN_DISPARITY everywhere: proposal cost exactly COST_FOR_INVALID
 LAM, TH = 2.0, 1.5                            # designed scenes: c01 = c10 = LAM * TH = 3 between FAR and any label below, c00 in {0, 1, 2}
 LEVELS = (3.0, 3.25, 3.5)                     # disparities of the designed scenes' current labels
-REPORT = dict(worst=0.0, moves=0, ties=0, phase_nodes=0)
 
 
 @pytest.fixture(scope="module")
 def devmem():
-    from test_gpu_parity import _TorchDeviceMemory
-    return _TorchDeviceMemory()
-
-
-def bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
-
-
-def cut_value(tr, cap, mask):
-    """Value of the cut `mask` (True = SOURCE side) of the graph (tr, cap), the float32 capacities summed exactly in double: a node outside
-    the mask pays its source arc max(tr, 0), a node inside pays its sink arc max(-tr, 0), an arc from inside to outside pays its capacity."""
-    terms = [np.where(mask, np.maximum(-tr, 0), np.maximum(tr, 0)).astype(np.float64).ravel()]
-    h, w = mask.shape
-    for fi, (dx, dy) in enumerate(ARCS):
-        xs, xd = slice(max(-dx, 0), w - max(dx, 0)), slice(max(dx, 0), w + min(dx, 0))
-        cut = mask[:h - dy, xs] & ~mask[dy:, xd]
-        terms.append(cap[fi][:h - dy, xs][cut].astype(np.float64))
-    return math.fsum(np.concatenate(terms))
-
-
-def assert_non_adjacent(regions):
-    """The moves of one step read their neighbours' labels: the cells must not touch, diagonals included."""
-    for i, (x, y, w, h) in enumerate(regions):
-        for (x2, y2, w2, h2) in regions[i + 1:]:
-            assert x2 > x + w or x > x2 + w2 or y2 > y + h or y > y2 + h2, ((x, y, w, h), (x2, y2, w2, h2))
+    return TorchDeviceMemory()
 
 
 def make_energy(guide, D=8, seed=0, windR=8):
@@ -75,78 +49,10 @@ def make_energy(guide, D=8, seed=0, windR=8):
 
 
 def make_plan(E, regions):
-    R, W, H = E.params.windR, E.width, E.height
-    fr = [(max(x - R, 0), max(y - R, 0), min(x + w + R, W) - max(x - R, 0), min(y + h + R, H) - max(y - R, 0)) for (x, y, w, h) in regions]
-    plan = E.make_plan(fr, regions)
+    from localexpstereo_b200.sweep import window_rects
+    plan = E.make_plan(window_rects(regions, E.params.windR, E.width, E.height), regions)
     plan.set_units(regions, np.arange(len(regions)))
     return plan
-
-
-def proposal_costs(E, plan, planes, mode, devmem):
-    """The image lexp_plan_gc_step evaluates its proposals into: the same plan's unary launch with image output and the validity check."""
-    d = devmem.zeros((E.height, E.width), fill=np.nan)
-    plan.eval_device(np.asarray(planes, np.float32), devmem.ptr(d), E.width * 4, with_check=True, mode=mode)
-    E.sync()
-    return np.array(devmem.download(d), np.float32)
-
-
-def certify_gc_step(E, plan, regions, mode, lam, th, devmem, planes=None, kind=0, m=0, seed=0, exact=False, ties_ok=False):
-    """One proposal step of `plan` (Plan.gc_step: PROP_LIST with `planes`, or a device proposer) checked move by move, (a) to (d) of the
-    module docstring.  Returns one record per cell.
-    Tolerance of (b) to (d): 1e-6 * max(mf, 1e-3).  (b) also allows the double rounding of konst (the device sums it per thread and per
-    block, the oracle per node and pairwise): 2 N u * (|konst| + mf + 8 N lam th) bounds any summation order of N terms whose
-    absolute values add up to at most that (a node's konst terms are >= -4 lam th).  exact: no tolerance at all."""
-    import localexpstereo_b200 as L
-    H, W = E.height, E.width
-    n = len(regions)
-    assert_non_adjacent(regions)
-    assert (kind == L.PROP_LIST) == (planes is not None)
-    pre_c, pre_l = E.pm_get(mode)
-    coeff = E.smooth_coeff(mode)
-    d_pl, d_fl = devmem.zeros((n, 4)), devmem.zeros((n, 2))
-    plan.gc_step(kind, m, seed, planes=planes, d_planes_out=devmem.ptr(d_pl), d_flows_out=devmem.ptr(d_fl), mode=mode)
-    E.sync()
-    post_c, post_l = E.pm_get(mode)
-    used = np.array(devmem.download(d_pl), np.float32)
-    flows = np.ascontiguousarray(devmem.download(d_fl)).view(np.float64)[:, 0].copy()
-    if planes is not None:
-        assert np.array_equal(bits(used), bits(np.reshape(planes, (n, 4))))
-    q_img = proposal_costs(E, plan, used, mode, devmem)
-    inside = np.zeros((H, W), bool)
-    cells = []
-    for i, reg in enumerate(regions):
-        x, y, w, h = (int(v) for v in reg)
-        sl = np.s_[y:y + h, x:x + w]
-        inside[sl] = True
-        q, l1, N = q_img[sl], used[i], w * h
-        tr, konst, cap = O.expansion_graph(pre_c, pre_l, q, l1, (x, y, w, h), coeff, lam, th)
-        mask_o, mf_o = c_oracle.grid_mincut(tr, cap)
-        old = (bits(post_c[sl]) == bits(pre_c[sl])) & (bits(post_l[sl]) == bits(pre_l[sl])).all(axis=2)
-        new = (bits(post_c[sl]) == bits(q)) & (bits(post_l[sl]) == bits(l1)).all(axis=2)
-        bad = ~(old | new)
-        assert not bad.any(), f"(a) cell {(x, y, w, h)}: {int(bad.sum())} pixels hold neither their pre-move state nor the proposal, e.g. {np.argwhere(bad)[0]}"
-        either = old & new      # the pre-move state is the proposal already: an isolated node with tr = 0, either side of the cut
-        mask_d = new
-        v_d, v_o = cut_value(tr, cap, mask_d), cut_value(tr, cap, mask_o)
-        tol = 0.0 if exact else 1e-6 * max(mf_o, 1e-3)
-        slack = 0.0 if exact else 2 * N * U * (abs(konst) + abs(mf_o) + 8 * N * lam * th)
-        err = abs((flows[i] - konst) - v_d)
-        diff = (mask_d != mask_o) & ~either
-        msg = (f"cell {(x, y, w, h)} ({N} nodes): device flow {flows[i]!r}, konst {konst!r}, oracle max flow {mf_o!r}, cut value of the "
-               f"device's mask {v_d!r}, of the oracle's {v_o!r}, {int(diff.sum())} nodes on different sides")
-        assert err <= tol + slack, "(b) " + msg
-        assert abs(v_d - v_o) <= tol, "(c) " + msg
-        assert abs(mf_o - v_o) <= tol + (0.0 if exact else 1e-7 * max(mf_o, 1e-3)), "oracle: " + msg
-        assert ties_ok or not diff.any(), "(d) " + msg
-        REPORT["worst"] = max(REPORT["worst"], err / max(mf_o, 1e-3))
-        REPORT["moves"] += 1
-        REPORT["ties"] += int(diff.sum())
-        cells.append(dict(region=(x, y, w, h), konst=konst, mf=mf_o, flow=float(flows[i]), mask=mask_d, q=q, ties=int(diff.sum()),
-                          err=err / max(mf_o, 1e-3), slack=slack))
-    out = ~inside
-    assert np.array_equal(bits(post_c[out]), bits(pre_c[out])) and np.array_equal(bits(post_l[out]), bits(pre_l[out])), \
-        "(a) a pixel outside the step's cells changed"
-    return cells
 
 
 # ---- designed (exact) scenes ---------------------------------------------------------------------------------------------------------
@@ -426,7 +332,7 @@ def test_every_move_of_a_natural_scene(devmem):
     recorded.  FP32 costs can tie: (d) only counts nodes on different sides, (a) to (c) hold on every move."""
     import lexp_golden
     import localexpstereo_b200 as L
-    from localexpstereo_b200.sweep import GCSweep, expand_proposers, pm_seed
+    from localexpstereo_b200.sweep import GCSweep
     G = lexp_golden.load()
     D = G["D"]
     lam, th = 1.0, 1.0
@@ -434,18 +340,13 @@ def test_every_move_of_a_natural_scene(devmem):
     props = [[(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 2)], [(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 1)]]
     S = GCSweep(E, unit_sizes=[6, 18], proposers=props, lam=lam, omega=10.0, th_smooth=th, epsilon=0.01)
     try:
-        rng = O.CvRNG(4)
         S.begin()
-        S.init(np.stack([O.create_random_label(rng, u[0] + rng.uniform_int(0, u[2]), u[1] + rng.uniform_int(0, u[3]), 0.0, D - 1.0)
-                         for u in S.init_units]))
+        S.init(seeded_labels(S, 4))
         n_moves = n_ties = 0
         worst = 0.0
         for g in S.groups:
-            lay = S.lm.layers[g.layer]
-            regions = [lay.sharedRegions[r] for r in g.cells]
-            for k, (kind, m) in enumerate(expand_proposers(props[g.layer], 0, D - 1.0)):
-                cells = certify_gc_step(E, g.plan, regions, 0, lam, th, devmem, kind=kind, m=m, seed=pm_seed(12, 0, 0, g.layer, g.group, k),
-                                        ties_ok=True)
+            for k, kind, m, sd in S.group_steps(g.layer, g.group, 0, 12):
+                cells = certify_gc_step(E, g.plan, g.targets, 0, lam, th, devmem, kind=kind, m=m, seed=sd, ties_ok=True)
                 n_moves += len(cells)
                 n_ties += sum(c["ties"] for c in cells)
                 worst = max([worst] + [c["err"] for c in cells])

@@ -5,15 +5,15 @@ state must be bit-identical to the one-CTA path.  LEXP_GC_BIG_NODES = 0 sends ev
 import numpy as np
 import pytest
 
-import test_gpu_zz_gc as G
+import lexp_replay as G
+from lexp_testlib import TorchDeviceMemory
 
 pytestmark = pytest.mark.gpu
 
 
 @pytest.fixture(scope="module")
 def devmem():
-    from test_gpu_parity import _TorchDeviceMemory
-    return _TorchDeviceMemory()
+    return TorchDeviceMemory()
 
 
 def test_phase_kernels_equal_the_one_cta_path(devmem, monkeypatch):

@@ -26,7 +26,7 @@ import pytest
 
 from oracle import c_oracle
 from oracle import lexp_oracle as O
-from lexp_testlib import assert_costs_close, make_scene
+from lexp_testlib import TorchDeviceMemory, assert_costs_close, bits, make_scene, seeded_labels
 
 pytestmark = pytest.mark.gpu
 
@@ -35,12 +35,7 @@ INVALID = np.float32(O.COST_FOR_INVALID)
 
 @pytest.fixture(scope="module")
 def devmem():
-    from test_gpu_parity import _TorchDeviceMemory
-    return _TorchDeviceMemory()
-
-
-def bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
+    return TorchDeviceMemory()
 
 
 def ulps(a, b):
@@ -62,20 +57,6 @@ class Tally:
                 f"Random within tolerance {self.random} of {self.n_random} ({frac:.4f} bit-identical); source pixels named by their tag "
                 f"{self.named} of {self.n_named}; worst q err vs the FP64 oracle {self.worst_q:.2e}; (I) PM = unary instantiation: "
                 f"{'held' if self.instantiations_agree else 'FAILED'}; {self.t_step:.1f} s certifying, {self.t_oracle:.1f} s of it in the C oracle")
-
-
-def cells_of(S, li, cells):
-    """unit, target and filter rects and global cell ids of `cells` of layer li of the PMSweep S, in call order."""
-    lay = S.lm.layers[li]
-    base = sum(len(l.unitRegions) for l in S.lm.layers[:li])
-    return ([lay.unitRegions[r] for r in cells], [lay.sharedRegions[r] for r in cells], [lay.filterRegions[r] for r in cells],
-            [base + int(r) for r in cells])
-
-
-def init_cells(S):
-    R, W, H = S.energy.params.windR, S.energy.width, S.energy.height
-    fr = [(max(x - R, 0), max(y - R, 0), min(x + w + R, W) - max(x - R, 0), min(y + h + R, H) - max(y - R, 0)) for (x, y, w, h) in S.init_units]
-    return list(S.init_units), list(S.init_units), fr, [int(i) for i in S.init_index]
 
 
 class Rig:
@@ -152,13 +133,13 @@ class Rig:
         self.Eq.sync()
         return self.get(self.Eq, "q")
 
-    def certify(self, plan, qplan, cells, kind, m=0, seed=0, step_index=0, init=False, planes=None, sync=None):
-        """One step of `plan` (qplan: the twin's plan of the same cells) checked by (P), (U), (Q) and (I) of the module docstring.
+    def certify(self, g, qplan, kind, m=0, seed=0, step_index=0, init=False, planes=None, sync=None):
+        """One step of the GroupPlan g (qplan: the twin's plan of the same cells) checked by (P), (U), (Q) and (I) of the module docstring.
         Returns (pre, post, inside, q): the states are views of buffers the next step overwrites; inside marks the target pixels,
         q holds their proposal costs."""
         L, E, dm, T = self.L, self.E, self.dm, self.T
         t0 = time.perf_counter()
-        units, targets, filters, ids = cells
+        plan, units, targets, filters, ids = g.plan, g.units, g.targets, g.filters, g.ids
         n = plan.num_calls
         assert len(units) == n and (kind == L.PROP_LIST) == (planes is not None)
         pre_c, pre_l = self.get(E, "pre")
@@ -235,39 +216,34 @@ class Rig:
         T.t_step += time.perf_counter() - t0
         return (pre_c, pre_l), (post_c, post_l), inside, q
 
-    # ---- the schedule of PMSweep.init / iteration_by_group, one step at a time ------------------------------------------------------
+    # ---- the sweep's own walk (PMSweep.init / iteration_by_group), one step at a time ----------------------------------------------
     def init(self, labels, certify=True):
-        S = self.S
-        self.E.pm_reset_sync()
-        if certify:
-            self.certify(S.init_plan, self.Sq.init_plan, init_cells(S), self.L.PROP_LIST, planes=np.asarray(labels, np.float32), init=True,
-                         sync=S.clock.sync_args(True, True))
-        else:
-            S.init_plan.pm_step(0, self.L.PROP_LIST, planes=labels, init=True, mode=self.mode, **S.clock.sync_args(True, True))
-        S.clock.group_done(S.init_owners)
-        S._advance()
+        def issue(g, steps):
+            ((k, kind, _, _, sync),) = steps
+            if certify:
+                self.certify(g, self.Sq.init_plan, kind, planes=np.asarray(labels, np.float32), init=True, sync=sync)
+            else:
+                g.plan.pm_step(k, kind, planes=labels, init=True, mode=self.mode, **sync)
+        for _ in self.S.walk(None, 0, issue):
+            pass
 
     def iteration(self, it, seed, certify=lambda li: True, snap_layer=None):
         """One iteration of the sweep under test; steps of the layers `certify` selects are certified.  Returns the state at the end
         of layer snap_layer (None: not taken)."""
-        from localexpstereo_b200.sweep import expand_proposers, pm_seed
-        S, E, snap = self.S, self.E, None
-        E.pm_reset_sync()
-        for n, ((li, gi, g, owners), (_, _, gq, _)) in enumerate(zip(S.schedule, self.Sq.schedule)):
-            steps = expand_proposers(S.proposers[li], it, E.MAX_DISPARITY, E.MIN_DISPARITY)
-            for k, (kind, m) in enumerate(steps):
-                sd = pm_seed(seed, S.mode, it, li, gi, k)
-                sync = S.clock.sync_args(k == 0, k == len(steps) - 1)
-                if certify(li):
-                    self.certify(g.plan, gq.plan, cells_of(S, li, g.cells), kind, m, sd, k, sync=sync)
+        S, snap = self.S, None
+        twin = {(g.layer, g.group): g.plan for g in self.Sq.groups}
+
+        def issue(g, steps):
+            for k, kind, m, sd, sync in steps:
+                if certify(g.layer):
+                    self.certify(g, twin[(g.layer, g.group)], kind, m, sd, k, sync=sync)
                 else:
                     g.plan.pm_step(k, kind, m, sd, mode=self.mode, **sync)
-            S.clock.group_done(owners if steps else [])
+        for n, _ in enumerate(S.walk(it, seed, issue)):
+            li = S.schedule[n][0]
             if li == snap_layer and (n + 1 == len(S.schedule) or S.schedule[n + 1][0] != li):
-                snap = self.get(E)
-        S._advance()
+                snap = self.get(self.E)
         return snap
-
 
     def twin_reference(self, labels, seed, upto, tag=False):
         """The twin's uninterrupted sweep (PMSweep.init / iteration_by_group): the state after the initialisation (upto = None) or
@@ -291,12 +267,6 @@ class Rig:
 def assert_same_state(a, b, what):
     assert np.array_equal(bits(a[0]), bits(b[0])), f"{what}: currentCost differs at {int((bits(a[0]) != bits(b[0])).sum())} pixels"
     assert np.array_equal(bits(a[1]), bits(b[1])), f"{what}: currentLabeling differs"
-
-
-def init_labels(S, D, seed, MIN=0.0, MAX=None):
-    rng = O.CvRNG(seed)
-    MAX = D - 1.0 if MAX is None else MAX
-    return np.stack([O.create_random_label(rng, u[0] + rng.uniform_int(0, u[2]), u[1] + rng.uniform_int(0, u[3]), MIN, MAX) for u in S.init_units])
 
 
 def run_sweep(R, labels, iterations, seed, tag=True, what="scene"):
@@ -331,7 +301,7 @@ def scene_tags(devmem, mode=0):
         for lay in R.S.lm.layers:
             us = lay.unitRegions
             assert min(u[2] for u in us) < lay.regionUnitSize and min(u[3] for u in us) < lay.regionUnitSize, "the image should be ragged"
-        T = run_sweep(R, init_labels(R.S, D, 21), 2, 5, what=f"pixel tags, mode {mode}")
+        T = run_sweep(R, seeded_labels(R.S, 21), 2, 5, what=f"pixel tags, mode {mode}")
         assert T.n_exact > 300 and T.n_random > 300 and T.named > 0
         return T
     finally:
@@ -347,8 +317,7 @@ def scene_update_edges(devmem, mode=0):
     try:
         S = R.S
         R.Eq.pm_begin(mode)
-        (li, gi, g, _), (_, _, gq, _) = S.schedule[5], R.Sq.schedule[5]
-        cells = cells_of(S, li, g.cells)
+        (_, _, g, _), (_, _, gq, _) = S.schedule[5], R.Sq.schedule[5]
         n = g.plan.num_calls
         old = np.zeros((H, W, 4), np.float32)
         old[..., 2] = 3.0
@@ -360,7 +329,7 @@ def scene_update_edges(devmem, mode=0):
         def step(cost, planes):
             R.E.pm_reset_sync()
             R.E.pm_begin(mode, cost, old)
-            pre, post, inside, q = R.certify(g.plan, gq.plan, cells, L.PROP_LIST, planes=planes)
+            pre, post, inside, q = R.certify(g, gq.plan, L.PROP_LIST, planes=planes)
             changed = (bits(post[0]) != bits(pre[0])) | (bits(post[1]) != bits(pre[1])).any(axis=2)
             return inside, q, changed
 
@@ -390,7 +359,7 @@ def scene_min_max(devmem, mn, mx):
     R = small_rig(devmem, H, W, D, 12, [8, 20], [[(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 3)], [(L.PROP_EXPANSION, 1), (L.PROP_RANDOM, 2)]],
                   seed=77, MIN=mn, MAX=mx)
     try:
-        run_sweep(R, init_labels(R.S, D, 13, mn, mx), 1, 9, what=f"MIN {mn}, MAX {mx}")
+        run_sweep(R, seeded_labels(R.S, 13), 1, 9, what=f"MIN {mn}, MAX {mx}")
     finally:
         R.close()
 
@@ -405,27 +374,27 @@ def scene_many_items(devmem):
     try:
         items = [g.plan.num_items / g.plan.num_calls for g in R.S.groups if g.layer == 1]
         assert min(items) >= 32, items
-        run_sweep(R, init_labels(R.S, D, 17), 1, 3, what=f"{min(items):.0f} work items per layer-1 cell")
+        run_sweep(R, seeded_labels(R.S, 17), 1, 3, what=f"{min(items):.0f} work items per layer-1 cell")
     finally:
         R.close()
 
 
 def scene_random_m(devmem, mode=1):
-    """Direct RandomProposer steps with m = 0, 1 and 120 (the C-ABI's bound: exp2f(-121) is still a normal float) on a tagged state."""
+    """Direct RandomProposer steps with m = 0, 1 and 120 (the C-ABI's bound: exp2f(-121) is still a normal float) on a tagged state,
+    with the random streams of the sweep's three RandomProposer steps of iteration 0 (seed 8)."""
     import localexpstereo_b200 as L
-    from localexpstereo_b200.sweep import pm_seed
     H, W, D = 44, 60, 12
-    R = small_rig(devmem, H, W, D, 12, [8], [[(L.PROP_EXPANSION, 1)]], mode, seed=6)
+    R = small_rig(devmem, H, W, D, 12, [8], [[(L.PROP_RANDOM, 3)]], mode, seed=6)
     try:
         S = R.S
         R.Eq.pm_begin(mode)
         R.E.pm_begin(mode)
-        R.init(init_labels(S, D, 31))
+        R.init(seeded_labels(S, 31))
         R.tag(R.E)
         for (li, gi, g, _), (_, _, gq, _) in list(zip(S.schedule, R.Sq.schedule))[:8]:
             R.E.pm_reset_sync()
-            for k, m in enumerate((0, 1, 120)):
-                R.certify(g.plan, gq.plan, cells_of(S, li, g.cells), L.PROP_RANDOM, m, pm_seed(8, mode, 0, li, gi, k), k)
+            for (k, kind, _, sd), m in zip(S.group_steps(li, gi, 0, 8), (0, 1, 120)):
+                R.certify(g, gq.plan, kind, m, sd, k)
         print(R.T.line(f"Random at m = 0, 1, 120, mode {mode}"))
         assert R.T.n_random > 80 and R.T.named > 0
     finally:
@@ -513,7 +482,7 @@ def scene_at_size(devmem, W, H, D, windR, mode, seed):
     R = Rig(devmem, imL, imR if mode else None, volL, volR if mode else None, windR, None, V3_PROPOSERS_DEVICE, mode)
     try:
         t0 = time.perf_counter()
-        run_sweep(R, init_labels(R.S, D, seed), 2, 1000 + seed, what=f"{W} x {H} x {D}, windR {windR}, mode {mode}")
+        run_sweep(R, seeded_labels(R.S, seed), 2, 1000 + seed, what=f"{W} x {H} x {D}, windR {windR}, mode {mode}")
         print(f"  {time.perf_counter() - t0:.1f} s in all")
     finally:
         R.close()

@@ -218,6 +218,16 @@ public:
             if ((int)labels.size() != numInitLabels()) throw std::invalid_argument("PatchMatchPhase: one label per unit region of layer 0");
             check(lexp_pm_sweep_init(sweep_, reinterpret_cast<const lexp_plane*>(labels.data())));
         }
+        // initCurrentFast started from a given labeling (FastGCStereo.h:116-130): currentLabeling_[mode] = labeling (H x W CV_32FC4,
+        // continuous) and, for every pixel p, currentCost_[mode](p) = ComputeUnaryPotential((p - windR, 2 windR + 1) & image, {p}, .,
+        // labeling(p)) -- one launch on the device instead of one blocking call per pixel.  Resumes or warm-starts a run.
+        // After postProcess, which changes the labels but not the costs, lexp_pm_init_from_labeling(ctx, mode) on each view recomputes
+        // currentCost_ for the post-processed labeling (then lexp_energy reports the data term of the final state).
+        void initFromLabeling(const cv::Mat& labeling) {
+            static_assert(sizeof(Plane) == sizeof(lexp_plane), "Plane must stay {a,b,c,v} floats (Plane.h:4-8)");
+            check(lexp_pm_begin(ctx_, mode_, nullptr, reinterpret_cast<const lexp_plane*>(labeling.data)));
+            check(lexp_pm_init_from_labeling(ctx_, mode_));
+        }
         int iteration(int iteration, uint64_t seed) {
             int n = 0;
             check(lexp_pm_sweep_iteration(sweep_, iteration, seed, &n));

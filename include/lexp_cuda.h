@@ -283,6 +283,15 @@ LEXP_API int lexp_pairwise_terms(lexp_ctx* ctx, int mode, int n, const lexp_rect
  * into lexp_plan_pm_step(.., LEXP_PM_INIT); this form also serves the image-based energy (`-mode MiddV2`), whose iterations are all
  * graph-cut iterations.  Asynchronous, stream ordered (host planes are staged before the call returns). */
 LEXP_API int lexp_plan_init_step(lexp_ctx* ctx, lexp_plan* plan, int mode, const lexp_plane* planes, int planes_on_device);
+/* initCurrentFast started from a given labeling (FastGCStereo.h:116-130), for any energy kind: for every pixel p of view `mode`,
+ * currentCost(p) = ComputeUnaryPotential(F(p), {p}, ., currentLabeling(p)) with F(p) = (p.x - windR, p.y - windR, 2 windR + 1, 2 windR + 1)
+ * clipped to the image, the check version (IsValiLabel's 1x1 path: COST_FOR_INVALID where it fails).  The labeling is the one the state
+ * holds, from lexp_pm_begin(ctx, mode, NULL, labeling) or written through lexp_pm_device_state, and is not changed.  Use it to resume or
+ * warm-start a run from a labeling, and to recompute the costs after lexp_post_process, which changes the labels only.  Asynchronous on
+ * the context's stream and graph-capturable (one launch); later launches on the stream see its writes.  On a connected cell shard each
+ * rank computes the whole image into its own copy (no peer stores): call it on every rank with the same labeling.  LEXP_ERR_STATE
+ * before lexp_pm_begin or without the view's inputs, LEXP_ERR_INVALID for a bad mode; on error nothing is enqueued.  DESIGN.md 3g. */
+LEXP_API int lexp_pm_init_from_labeling(lexp_ctx* ctx, int mode);
 /* The reference's cost-volume file, raw float[ndisp][height][width] without a header (`loadMatBinary(.., "im0.acrt", volL, false)`,
  * main.cpp:353-358,364), streamed from disk in slabs through page-locked buffers with the volume preparation `transform`
  * (LEXP_VOL_*) fused in as for lexp_set_volume_host_ex: the 17 GB volume of the 4K configuration never exists in host memory. */

@@ -83,6 +83,7 @@ SYMBOLS = {
     "lexp_get_smooth_coeff": (C.c_int, [_P, C.c_int, _P]),
     "lexp_pairwise_terms": (C.c_int, [_P, C.c_int, C.c_int, _P, _P, _P]),
     "lexp_plan_init_step": (C.c_int, [_P, _P, C.c_int, _P, C.c_int]),
+    "lexp_pm_init_from_labeling": (C.c_int, [_P, C.c_int]),
     "lexp_set_volume_file": (C.c_int, [_P, C.c_int, C.c_char_p, C.c_int]),
     "lexp_get_disparities": (C.c_int, [_P, C.c_int, _P]),
     "lexp_save_pfm": (C.c_int, [C.c_char_p, _P, C.c_int, C.c_int, C.c_ssize_t]),

@@ -6,6 +6,7 @@
 #include "lexp_gc.cuh"
 #include "lexp_post.cuh"
 #include "lexp_ransac.cuh"
+#include "lexp_label_cost.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -158,6 +159,7 @@ struct lexp_ctx {
     size_t smem_limit = 0;
     size_t window_max = 0;
     bool smem_configured[2] = {false, false};
+    bool lc_smem_configured[2] = {false, false};   // lexp_label_cost_kernel<NAIVE>: dynamic shared memory opt-in done
     bool own_stream = true;
     bool vol_finite[2] = {false, false};
     // single-cell plans of lexp_eval_cell, keyed by (filterRect, targetRect): the unchanged reference loop calls the
@@ -1577,6 +1579,39 @@ int lexp_plan_init_step(lexp_ctx* c, lexp_plan* pl, int mode, const lexp_plane* 
     const int W = c->p.width;
     { int rc = run_plan(c, pl, mode, dp, c->d_prop_cost[mode], W, 0, 1); if (rc) return rc; }   // ComputeUnaryPotential (:111)
     LEXP_CUDA(launch_aux(c, lexp_gc_assign_kernel, pl->ncalls, 256, pl->d_gc_cells, dp, c->d_prop_cost[mode], c->d_cur_cost[mode], c->d_cur_label[mode], W));
+    return LEXP_OK;
+}
+
+// initCurrentFast started from the labeling the state holds (FastGCStereo.h:116-130): lexp_label_cost.cuh, one ordinary stream-ordered
+// launch (launch_aux_smem clears chain_ok, so the next fused launch does not overlap it and reads the costs it wrote).  Writes only this
+// rank's copy of currentCost_.
+int lexp_pm_init_from_labeling(lexp_ctx* c, int mode) {
+    if (!c || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    LEXP_ENTER(c);
+    const bool naive = c->p.energy_kind == 1;
+    if (naive) {
+        if (!c->d_exi[0] || !c->d_exi[1]) return fail(LEXP_ERR_STATE, "NaiveStereoEnergy needs the images of both views");
+    } else if (!c->d_guide[mode] || !c->d_vol[mode]) return fail(LEXP_ERR_STATE, "image / volume of this view not set");
+    const int H = c->p.height, W = c->p.width;
+    if (H > 65535) return fail(LEXP_ERR_INVALID, "lexp_pm_init_from_labeling: image taller than 65535 rows");
+    const size_t smem = label_cost_smem_bytes(c->R);
+    if (smem > c->smem_limit) return fail(LEXP_ERR_INVALID, "lexp_pm_init_from_labeling needs more shared memory than the device offers");
+    LcParams lp{};
+    lp.vol = c->d_vol[mode]; lp.Wb = (W + 3) / 4;
+    lp.guide = c->d_guide[mode]; lp.statA = c->d_statA[mode]; lp.statB = c->d_statB[mode]; lp.statC = c->d_statC[mode];
+    lp.exi_own = c->d_exi[mode]; lp.exi_other = c->d_exi[1 - mode];
+    lp.label = c->d_cur_label[mode]; lp.cost = c->d_cur_cost[mode];
+    lp.H = H; lp.W = W; lp.D = c->p.ndisp; lp.R = c->R; lp.windR = c->p.windR; lp.mode = mode;
+    lp.th_col = c->p.th_col; lp.min_disp = c->p.min_disp; lp.max_disp = c->p.max_disp;
+    lp.thresh_color = c->p.th_col * (1.0f - c->p.alpha);    // StereoEnergy.h:663
+    lp.thresh_gradient = c->p.th_grad * c->p.alpha;          // StereoEnergy.h:664
+    auto kern = naive ? lexp_label_cost_kernel<true> : lexp_label_cost_kernel<false>;
+    if (!c->lc_smem_configured[naive]) {
+        LEXP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_limit));
+        c->lc_smem_configured[naive] = true;
+    }
+    LEXP_CUDA(launch_aux_smem(c, kern, dim3((unsigned)W, (unsigned)H), kLcThreads, smem, lp));
     return LEXP_OK;
 }
 

@@ -393,6 +393,13 @@ class CostVolumeEnergy:
         assert l is None or l.shape == (self.height, self.width, 4)
         check(lib().lexp_pm_begin(self._h, mode, None if c is None else c.ctypes.data, None if l is None else l.ctypes.data))
 
+    def pm_init_from_labeling(self, mode=0):
+        """initCurrentFast started from a given labeling (FastGCStereo.h:116-130): currentCost_[mode](p) = ComputeUnaryPotential(
+        (p - windR, 2 windR + 1) & image, {p}, ., currentLabeling_[mode](p)) for every pixel, from the labeling the state holds
+        (pm_begin(mode, labeling=...) or written through pm_device_state).  The labeling is unchanged.  Asynchronous on the context's
+        stream.  Also recomputes the costs after post_process, which changes only the labels."""
+        check(lib().lexp_pm_init_from_labeling(self._h, int(mode)))
+
     def pm_get(self, mode=0, want_cost=True, want_labeling=True, out_cost=None, out_labeling=None):
         """Copies the state back; `out_cost` / `out_labeling`: caller's (e.g. page-locked) arrays to fill instead of new ones."""
         cost = out_cost if out_cost is not None else (np.empty((self.height, self.width), np.float32) if want_cost else None)

@@ -183,6 +183,8 @@ public:
     // A maintainer replaces the pm loop of run() by (INTEGRATION.md section 4):
     //     CudaCostVolumeEnergy::PatchMatchPhase pm(energy, mode, {5, 15, 25}, {{{LEXP_PROP_EXPANSION, 1}, {LEXP_PROP_RANSAC, 1}, {LEXP_PROP_RANDOM, 7}}, ...});
     //     pm.begin(); pm.init(labels); for (it < pmInit) pm.iteration(it, seed); pm.get(currentCost_[mode], currentLabeling_[mode]);
+    // Both energies: with CudaNaiveStereoEnergy (`-mode MiddV2`, single GPU) the whole run of main.cpp:310-312 is begin, init,
+    // iteration x 2 (pmIterations), graphCutIteration x 5, disparities, savePfm.
     class PatchMatchPhase {
         lexp_ctx* ctx_;
         lexp_pm_sweep* sweep_ = nullptr;
@@ -273,6 +275,8 @@ private:
 // NaiveStereoEnergy (StereoEnergy.h:629-764) on the device: the image-based unary term of `-mode MiddV2`.  The reference builds it
 // inside the PMStereoBase constructor (PMStereoBase.h:37); replace it the same way as above:
 //     stereo.setStereoEnergyCPU(std::make_unique<CudaNaiveStereoEnergy>(imL, imR, param, maxdisp));
+// or run the demo's whole optimisation on the device (main.cpp:310-312, INTEGRATION.md section 4b) with a PatchMatchPhase on it, layers
+// {5, 15, 25}: begin, init, iteration x 2, graphCutIteration x 5, disparities, savePfm.
 class CudaNaiveStereoEnergy : public CudaCostVolumeEnergy {
 public:
     CudaNaiveStereoEnergy(const cv::Mat imL, const cv::Mat imR, Parameters params, float MAX_DISPARITY, float MIN_DISPARITY = 0,

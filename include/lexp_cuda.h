@@ -185,7 +185,10 @@ LEXP_API int lexp_combine_stats(const lexp_ctx* ctx, int64_t* batches, int64_t* 
  * and step) and the update fused into the epilogue of the unary-cost kernel: nothing crosses PCIe between steps.  The proposal steps
  * of a cell are ordered by per-cell completion counters, so consecutive launches overlap on the device.  A LEXP_PROP_RANSAC step is
  * one launch more: the RANSAC fit of every cell into the plan's plane buffer, ordered after every earlier launch of the stream, which
- * the step's own launch then reads like a list. */
+ * the step's own launch then reads like a list.
+ * Both energy kinds: the cost-volume energy, and the image-based energy (NaiveStereoEnergy, `-mode MiddV2`: its two pm iterations
+ * run here, main.cpp:21,310-312) on one GPU -- a view of that energy connected to peers (lexp_pm_ipc_connect / lexp_pm_connect_local)
+ * gets LEXP_ERR_INVALID from lexp_plan_pm_step[_ex] and nothing is enqueued.  The image-based energy needs the images of both views. */
 #define LEXP_PROP_LIST 0       /* planes supplied by the caller (host list replay) */
 #define LEXP_PROP_EXPANSION 1  /* ExpansionProposer::getNextProposal */
 #define LEXP_PROP_RANDOM 2     /* RandomProposer::getNextProposal, m = outerIter + iter */
@@ -248,7 +251,8 @@ LEXP_API int lexp_pm_advance_epoch(lexp_ctx* ctx, int mode, int delta);
  * LEXP_PROP_RANSAC; a LEXP_PROP_LIST slot is not allowed here -- use lexp_plan_pm_step for replays), and the epoch bookkeeping of the
  * group boundaries.  LEXP_PROP_RANSAC only with K = 1 (K > 1 would need the snapshot of startIterations to outlive the step) and
  * world = 1 (the cell shard has no RANSAC support); otherwise LEXP_ERR_INVALID.
- * rank / world: the multi-GPU cell shard (0 / 1 on a single GPU); connect the contexts first (lexp_pm_ipc_connect). */
+ * rank / world: the multi-GPU cell shard (0 / 1 on a single GPU); connect the contexts first (lexp_pm_ipc_connect).
+ * Both energy kinds; the image-based energy on one GPU only (world = 1, not connected to peers). */
 typedef struct lexp_pm_sweep lexp_pm_sweep;
 LEXP_API int lexp_pm_sweep_create(lexp_ctx* ctx, int mode, int n_layers, const int* unit_sizes, const int* n_proposers,
                                   const int* proposer_kind, const int* proposer_K, int rank, int world, lexp_pm_sweep** out);
@@ -256,7 +260,8 @@ LEXP_API int lexp_pm_sweep_destroy(lexp_pm_sweep* sweep);
 /* number of unit regions of layer 0 (= labels lexp_pm_sweep_init expects) */
 LEXP_API int lexp_pm_sweep_num_init_labels(const lexp_pm_sweep* sweep);
 /* initCurrentFast (FastGCStereo.h:101-113) with one label per unit region of layer 0 (all of them, in LayerManager order; a rank of
- * a cell shard evaluates its share).  lexp_pm_begin first.  Asynchronous. */
+ * a cell shard evaluates its share).  lexp_pm_begin first.  Asynchronous for the cost-volume energy (a LEXP_PM_INIT step); the
+ * image-based energy takes the lexp_plan_init_step form and returns after its launches have completed. */
 LEXP_API int lexp_pm_sweep_init(lexp_pm_sweep* sweep, const lexp_plane* labels_host);
 /* One pm iteration over all layers (FastGCStereo.h:147-157, doGC == false): every cell of every group visited with its layer's
  * proposers, RandomProposer with m = iteration + iter and its early stop (Proposer.h:149-152).  Asynchronous; returns the number
@@ -280,8 +285,9 @@ LEXP_API int lexp_get_smooth_coeff(lexp_ctx* ctx, int mode, float* out8_host);
 LEXP_API int lexp_pairwise_terms(lexp_ctx* ctx, int mode, int n, const lexp_rect* regions, const lexp_plane* planes, float* out_host);
 /* initCurrentFast for any energy kind (FastGCStereo.h:101-113): for every call of the plan, currentLabeling(targetRect) = planes[call] and
  * currentCost(targetRect) = its unary cost (ComputeUnaryPotential on the call's filterRect).  The cost-volume energy has the same step fused
- * into lexp_plan_pm_step(.., LEXP_PM_INIT); this form also serves the image-based energy (`-mode MiddV2`), whose iterations are all
- * graph-cut iterations.  Asynchronous, stream ordered (host planes are staged before the call returns). */
+ * into lexp_plan_pm_step(.., LEXP_PM_INIT); lexp_pm_sweep_init uses this form for the image-based energy (`-mode MiddV2`), whose run
+ * then continues with its pm iterations (lexp_pm_sweep_iteration) and its graph-cut iterations.  Asynchronous, stream ordered (host
+ * planes are staged before the call returns). */
 LEXP_API int lexp_plan_init_step(lexp_ctx* ctx, lexp_plan* plan, int mode, const lexp_plane* planes, int planes_on_device);
 /* initCurrentFast started from a given labeling (FastGCStereo.h:116-130), for any energy kind: for every pixel p of view `mode`,
  * currentCost(p) = ComputeUnaryPotential(F(p), {p}, ., currentLabeling(p)) with F(p) = (p.x - windR, p.y - windR, 2 windR + 1, 2 windR + 1)

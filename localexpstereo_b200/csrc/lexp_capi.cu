@@ -327,6 +327,12 @@ int launch_fused_t(lexp_ctx* c, const KParams& kp_in, int nitems, size_t smem, b
 int launch_fused(lexp_ctx* c, const KParams& kp, int nitems, size_t smem, bool allow_pdl = true) {
     if (smem > c->smem_limit) return fail(LEXP_ERR_INVALID, "tile needs more shared memory than the device offers");
     if (c->p.energy_kind == 1) {
+        if (kp.pm_mode) {   // PatchMatch phase of the image-based energy: the prologue's proposal feeds the inverse affine map
+            switch (c->R) {
+                case 10: return launch_fused_t<10, true, true>(c, kp, nitems, smem, allow_pdl);
+                default: return launch_fused_t<0, true, true>(c, kp, nitems, smem, allow_pdl);
+            }
+        }
         switch (c->R) {
             case 10: return launch_fused_t<10, true, false>(c, kp, nitems, smem, allow_pdl);
             default: return launch_fused_t<0, true, false>(c, kp, nitems, smem, allow_pdl);
@@ -1365,7 +1371,8 @@ int lexp_plan_pm_step_ex(lexp_ctx* c, lexp_plan* pl, int mode, int step_index, i
     if (kind == LEXP_PROP_RANSAC && (flags & LEXP_PM_INIT)) return fail(LEXP_ERR_INVALID, "LEXP_PROP_RANSAC cannot initialise: it fits the current state");
     if (!pl->d_calls || pl->sync_off < 0) return fail(LEXP_ERR_STATE, "lexp_plan_set_units has not been called for this plan");
     { int rc = require_pm_state(c, mode); if (rc) return rc; }
-    if (c->p.energy_kind != 0) return fail(LEXP_ERR_INVALID, "the device PatchMatch phase is implemented for the cost-volume energy");
+    if (c->p.energy_kind != 0 && c->peers[mode].world > 1)
+        return fail(LEXP_ERR_INVALID, "the image-based energy's PatchMatch phase runs on one GPU: this view is connected to peers");
     if (publish_epoch < 0 || (wait_mask >> kMaxPeers) || (wait_mask && !wait_epochs)) return fail(LEXP_ERR_INVALID, "bad epoch / mask");
     LEXP_ENTER(c);
     const Plane4* dp = nullptr;   // the other kinds: the device proposers generate the planes
@@ -1966,7 +1973,9 @@ int lexp_pm_sweep_init(lexp_pm_sweep* s, const lexp_plane* labels) {
     if (s->init_plan) {
         std::vector<lexp_plane> mine;
         for (int r : s->init_index) mine.push_back(labels[r]);
-        if (s->ctx->p.energy_kind != 0) {   // the image-based energy has no PatchMatch-phase kernel: unary launch + assignment (single GPU)
+        // the image-based energy initialises with a unary launch + assignment (single GPU).  Its last launch is an ordinary one
+        // (launch_aux clears chain_ok), as is lexp_pm_reset_sync's memset, so the first PatchMatch launch after it is stream-ordered
+        if (s->ctx->p.energy_kind != 0) {
             if (s->world != 1) return fail(LEXP_ERR_INVALID, "the image-based energy runs on one GPU");
             rc = lexp_plan_init_step(s->ctx, s->init_plan, s->mode, mine.data(), 0);
             if (rc == LEXP_OK) rc = lexp_sync(s->ctx);   // `mine` is local and pageable

@@ -201,7 +201,7 @@ __global__ void lexp_gc_propose_kernel(const CallInfo* __restrict__ calls, int n
 
 // initCurrentFast for any energy (FastGCStereo.h:101-113): `currentLabeling(unit) = label; ComputeUnaryPotential(.., currentCost(filterRegion), ..)`
 // -- after the fused kernel has written the unary costs of the cells' labels into the proposalCost image, every cell's region takes them
-// unconditionally.  One CTA per cell.  (The cost-volume energy has this fused into its PatchMatch-phase kernel, pm_mode 2.)
+// unconditionally.  One CTA per cell.  (The PatchMatch-phase kernel has this fused in, pm_mode 2.)
 __global__ void lexp_gc_assign_kernel(const GcCell* __restrict__ cells, const Plane4* __restrict__ planes, const float* __restrict__ prop_cost,
                                       float* __restrict__ cur_cost, float4* __restrict__ cur_label, int W) {
     const GcCell c = cells[blockIdx.x];

@@ -483,6 +483,8 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
         pl = s_pl;
     }
     if (NAIVE) {
+        // the call's map: from its filterRect and its plane -- in the PatchMatch phase the step's proposal, which the block above
+        // left in s_pl (read after its barrier), so every work item of a cell builds the same map from the same bits (DESIGN.md 3b)
         if (tid == 0) naive_inverse_affine(it, pl, P.mode, s_iM);
         __syncthreads();
     }

@@ -317,7 +317,8 @@ class GCSweep(PMSweep):
         energy.set_smoothness(lam, omega, th_smooth, epsilon)
 
     def init(self, labels):
-        """initCurrentFast; the image-based energy has no PatchMatch-phase kernel and takes the unary launch + assignment form."""
+        """initCurrentFast; the image-based energy takes the unary launch + assignment form (lexp_plan_init_step), as the native sweep
+        object does for it.  Its pm iterations (`iteration`) run on the PatchMatch-phase kernel like the cost-volume energy's."""
         if getattr(self.energy, "ENERGY_KIND", 0) == 0:
             return super().init(labels)
         if self.init_plan is not None:

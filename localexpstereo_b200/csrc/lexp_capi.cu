@@ -158,7 +158,7 @@ struct lexp_ctx {
     size_t smem_cap = 0;         // upper bound on a work item's dynamic shared memory, 0: none (LEXP_SMEM_CAP)
     size_t smem_limit = 0;
     size_t window_max = 0;
-    bool smem_configured[2] = {false, false};
+    bool smem_configured[3] = {false, false, false};   // [PM], [2]: the lean build of the PatchMatch-phase kernel
     bool lc_smem_configured[2] = {false, false};   // lexp_label_cost_kernel<NAIVE>: dynamic shared memory opt-in done
     bool own_stream = true;
     bool vol_finite[2] = {false, false};
@@ -282,7 +282,7 @@ void report_trace(lexp_ctx* c, int nitems) {
 }
 #endif
 
-template <int R_T, bool NAIVE, bool PM>
+template <int R_T, bool NAIVE, bool PM, int MIN_CTAS = kMinCtas>
 int launch_fused_t(lexp_ctx* c, const KParams& kp_in, int nitems, size_t smem, bool allow_pdl) {
     KParams kp = kp_in;
 #if LEXP_TRACE
@@ -297,10 +297,11 @@ int launch_fused_t(lexp_ctx* c, const KParams& kp_in, int nitems, size_t smem, b
         kp.trace = c->d_trace;
     }
 #endif
-    auto kern = lexp_fused_kernel<R_T, NAIVE, PM>;
-    if (!c->smem_configured[PM]) {  // one R instantiation per context (and one more for the PatchMatch phase)
+    auto kern = lexp_fused_kernel<R_T, NAIVE, PM, MIN_CTAS>;
+    bool& configured = c->smem_configured[MIN_CTAS == kLeanCtas ? 2 : PM];
+    if (!configured) {  // one R instantiation per context (and one more for the PatchMatch phase, and its lean build at R = 10)
         LEXP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_limit));
-        c->smem_configured[PM] = true;
+        configured = true;
     }
 #ifndef LEXP_EMU
     if (c->pdl && allow_pdl && c->chain_ok) {  // programmatic dependent launch: see griddepcontrol in lexp_fused_kernel
@@ -339,8 +340,14 @@ int launch_fused(lexp_ctx* c, const KParams& kp, int nitems, size_t smem, bool a
         }
     }
     if (kp.pm_mode) {   // PatchMatch phase: proposal prologue + fused update epilogue compiled in
+        // R = 10: the lean build (3 CTAs per SM) when three of the launch's widest item fit in shared memory and the launch has more
+        // items than kMinCtas x #SM slots.  A launch that fits in those slots gains no warps from it, only fewer loads in flight per
+        // CTA (measured: a 240-item layer-2 launch of the 2048x1536 sweep ran 25 % slower lean).  Unary-cost launches keep the kMinCtas
+        // build: the lean one made bench.py's unary sweep 21 % slower.
+        const bool lean = fused_fits_lean(smem) && (int64_t)nitems > (int64_t)kMinCtas * c->num_sms;
         switch (c->R) {
-            case 10: return launch_fused_t<10, false, true>(c, kp, nitems, smem, allow_pdl);
+            case 10: return lean ? launch_fused_t<10, false, true, kLeanCtas>(c, kp, nitems, smem, allow_pdl)
+                                 : launch_fused_t<10, false, true>(c, kp, nitems, smem, allow_pdl);
             case 16: return launch_fused_t<16, false, true>(c, kp, nitems, smem, allow_pdl);
             default: return launch_fused_t<0, false, true>(c, kp, nitems, smem, allow_pdl);
         }
@@ -638,7 +645,7 @@ int lexp_create(const lexp_params* params, lexp_ctx** out_ctx) {
     c->tile_oh_fixed = getenv("LEXP_TILE_OH") != nullptr;
     c->num_sms = prop.multiProcessorCount;
     // kMinCtas CTAs must fit next to each other: 1 KB of every CTA's shared memory is reserved by the system.  With the
-    // default build (2 CTAs) no cap is needed: the widest tile needs ~93 KB.
+    // default build (2 CTAs) no cap is needed at R = 10: the widest tile needs ~76 KB (at R = 16 it needs ~117 KB: one CTA per SM).
     c->ctas_per_sm = env_int("LEXP_CTAS_PER_SM", kMinCtas);
     c->pdl = !env_int("LEXP_PDL_OFF", 0);
     c->combine = env_int("LEXP_COMBINE", 1) != 0;

@@ -43,6 +43,13 @@ constexpr int kCH = 2;                 // rows per pipeline chunk
 #endif
 constexpr int kMinCtas = 2;           // resident CTAs per SM the kernel is compiled for (register cap 65536 / (kMinCtas * kThreads))
 constexpr int kG = 6;                 // rows per gather batch of team A (one batch of loads in flight)
+// Lean build of the cost-volume PatchMatch-phase kernel at R = 10 (windR 20 / 21): compiled for three resident CTAs (<= 56 registers),
+// 50 % more warps per SM to hide the latency of the row pipeline.  Team A gathers 4 rows per batch (3 CTAs x 4 rows keep the bytes in
+// flight of 2 x 6), teams C and E hold one batch of loads instead of two.  launch_fused picks it for launches of more than
+// kMinCtas x #SM items that are narrow enough for three CTAs to fit in shared memory (fused_fits_lean); otherwise the kMinCtas build
+// is faster.
+constexpr int kLeanCtas = 3;
+constexpr size_t kSmemPerSm = 228 * 1024, kSmemReservedPerCta = 1024;   // sm_90: shared memory per SM, and the system's share per CTA
 constexpr float kCostInvalid = 1000000.0f;  // StereoEnergy.h:45
 constexpr int kMaxPeers = 8;                // GPUs of one NVSwitch domain that share a PatchMatch-phase state
 
@@ -141,12 +148,17 @@ __host__ __device__ inline int srow_stride(int vw) {
     int s = sidx(vw + kRun + 7) + 1;
     return s + ((12 - (s & 7)) & 7);  // == 4 (mod 8) float4 units: the 2 rows x 4 runs of a quarter-warp hit 8 bank groups
 }
+// the four double-buffered hand-off buffers, each row sized by the columns it holds: hb1 VW, ho1 and hb2 W2 = VW - 2R, ho2 ow = VW - 4R
+__host__ __device__ inline int handoff_f4(int vw, int R) {
+    return 2 * kCH * (srow_stride(vw) + 2 * srow_stride(vw - 2 * R) + srow_stride(vw - 4 * R));
+}
 __host__ __device__ inline size_t fused_smem_bytes(int vw, int oh, int R) {
     const int K = 2 * R + 1;
     const int vh = oh + 4 * R;
-    const int rows = 8 * kCH * srow_stride(vw);
+    const int rows = handoff_f4(vw, R);
     return (size_t)((K * vw + 1) / 2 + K * (vw - 2 * R) + rows + 3 * ((vh + 3) / 4) + 3) * 16 + 16;  // + 6 doubles (NAIVE: inverse affine map) + the plane slot (PatchMatch phase) at the very end
 }
+__host__ __device__ inline bool fused_fits_lean(size_t smem) { return kLeanCtas * (smem + kSmemReservedPerCta) <= kSmemPerSm; }
 
 // ---- (f32, f32) register-pair helpers ----------------------------------------------------------
 typedef unsigned long long u64;
@@ -367,8 +379,8 @@ __device__ __forceinline__ int ld_acquire(const int* p) {
 // Cost-volume samples: plain read-only loads that allocate in L1: the d0 / d0+1 samples of a 4-pixel block share 128-byte lines.
 __device__ __forceinline__ float ldg_stream(const float* p) { return __ldg(p); }
 
-template <int R_T, bool NAIVE, bool PM>
-__global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KParams P) {
+template <int R_T, bool NAIVE, bool PM, int MIN_CTAS = kMinCtas>
+__global__ void __launch_bounds__(kThreads, MIN_CTAS) lexp_fused_kernel(const KParams P) {
     const int R = R_T > 0 ? R_T : P.R;
     const int K = 2 * R + 1;
     LEXP_DYNAMIC_SMEM(smem_raw);
@@ -391,30 +403,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
     Plane4 pl;
     if (!PM) pl = P.planes[it.call];
     const int VW = it.ow + 4 * R;
-    const int X0 = it.ox0 - 2 * R;
     const int W2 = VW - 2 * R;
-    const int SW = srow_stride(VW);   // row stride of the four hand-off buffers (sized for hb1: VW columns)
-    const int fx1 = it.fx + it.fw, fy1 = it.fy + it.fh;
-    // streamed rows y = ys + v, v in [0, VHs): the dependency cone of the tile, minus leading rows above
-    // the filterRect (they are zero padding).  Rows >= fy1 are zero rows that flush the running sums.
-    const int ys = max(it.oy0 - 2 * R, it.fy);
-    const int VHs = it.oy0 + it.oh + 2 * R - ys;
-    const int vReal = min(VHs, fy1 - ys);                    // rows [0, vReal) lie inside the filterRect
-    const int vC0 = max(it.oy0 - R, it.fy) + R - ys;         // first v whose stage-1 centre row (y - R) is needed
-    const int vC1 = min(VHs, fy1 + R - ys);                  // centre rows >= fy1 are zero rows
-    const int vE0 = it.oy0 + 2 * R - ys;                     // first v whose stage-2 centre row (y - 2R) is an output row
-
-    uint2* ring1 = reinterpret_cast<uint2*>(smem);   // [K][VW] {p, packed guide}: the products are recomputed when a row leaves the window
-    F4* ring2 = smem + (K * VW + 1) / 2;              // [K][W2]
-    F4* hb1 = ring2 + K * W2;              // [2][CH][SW] stage-1 column sums   (index: column - X0)
-    F4* ho1 = hb1 + 2 * kCH * SW;          // [2][CH][SW] stage-1 box sums      (index: column - X0 - R)
-    F4* hb2 = ho1 + 2 * kCH * SW;          // [2][CH][SW] stage-2 column sums   (index: column - X0 - R)
-    F4* ho2 = hb2 + 2 * kCH * SW;          // [2][CH][SW] stage-2 box sums      (index: column - X0 - 2R)
-    float* s_invny = reinterpret_cast<float*>(ho2 + 2 * kCH * SW);  // [VHs] 1 / (#rows of the window inside filterRect)
-    float* s_dbase = s_invny + 4 * ((it.oh + 4 * R + 3) / 4);        // [VHs] b*y + c of the plane  (NAIVE: int X0 of the warp)
-    int* s_Y0 = reinterpret_cast<int*>(s_dbase + 4 * ((it.oh + 4 * R + 3) / 4));  // [VHs] NAIVE: fixed-point source row
-    double* s_iM = reinterpret_cast<double*>(s_Y0 + 4 * ((it.oh + 4 * R + 3) / 4));  // [6] NAIVE: inverse affine map of the call
-
     if (PM) {
         // PatchMatch phase.  (0) Group boundary: the previous group (this rank's and, on the multi-GPU cell shard, the peers') must
         // have finished -- its last launch stored an epoch flag when its last work item completed; all launches of an iteration are
@@ -476,12 +465,37 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
             s_pl = q;
         }
         {   // zero-fill (the box filter is zero padded, GuidedFilter.h:43 BORDER_CONSTANT) by warps 1.. meanwhile
-            const int total = (K * VW + 1) / 2 + K * W2 + 8 * kCH * SW;
+            const int total = (K * VW + 1) / 2 + K * W2 + handoff_f4(VW, R);
             if (tid >= 32) for (int i = tid - 32; i < total; i += kThreads - 32) smem[i] = f4zero();
         }
         __syncthreads();
         pl = s_pl;
     }
+    // Tile geometry and shared-memory layout (fused_smem_bytes): defined after the PatchMatch prologue, whose out-of-line proposer
+    // call would otherwise have to keep them alive (the lean build has no registers to spare for that)
+    const int X0 = it.ox0 - 2 * R;
+    const int fx1 = it.fx + it.fw, fy1 = it.fy + it.fh;
+    // streamed rows y = ys + v, v in [0, VHs): the dependency cone of the tile, minus leading rows above
+    // the filterRect (they are zero padding).  Rows >= fy1 are zero rows that flush the running sums.
+    const int ys = max(it.oy0 - 2 * R, it.fy);
+    const int VHs = it.oy0 + it.oh + 2 * R - ys;
+    const int vReal = min(VHs, fy1 - ys);                    // rows [0, vReal) lie inside the filterRect
+    const int vC0 = max(it.oy0 - R, it.fy) + R - ys;         // first v whose stage-1 centre row (y - R) is needed
+    const int vC1 = min(VHs, fy1 + R - ys);                  // centre rows >= fy1 are zero rows
+    const int vE0 = it.oy0 + 2 * R - ys;                     // first v whose stage-2 centre row (y - 2R) is an output row
+
+    const int SW1 = srow_stride(VW), SW2 = srow_stride(W2), SWo = srow_stride(it.ow);   // row strides of the hand-off buffers
+    uint2* ring1 = reinterpret_cast<uint2*>(smem);   // [K][VW] {p, packed guide}: the products are recomputed when a row leaves the window
+    F4* ring2 = smem + (K * VW + 1) / 2;              // [K][W2]
+    F4* hb1 = ring2 + K * W2;              // [2][CH][SW1] stage-1 column sums   (index: column - X0)
+    F4* ho1 = hb1 + 2 * kCH * SW1;         // [2][CH][SW2] stage-1 box sums      (index: column - X0 - R)
+    F4* hb2 = ho1 + 2 * kCH * SW2;         // [2][CH][SW2] stage-2 column sums   (index: column - X0 - R)
+    F4* ho2 = hb2 + 2 * kCH * SW2;         // [2][CH][SWo] stage-2 box sums      (index: column - X0 - 2R)
+    float* s_invny = reinterpret_cast<float*>(ho2 + 2 * kCH * SWo);  // [VHs] 1 / (#rows of the window inside filterRect)
+    float* s_dbase = s_invny + 4 * ((it.oh + 4 * R + 3) / 4);        // [VHs] b*y + c of the plane  (NAIVE: int X0 of the warp)
+    int* s_Y0 = reinterpret_cast<int*>(s_dbase + 4 * ((it.oh + 4 * R + 3) / 4));  // [VHs] NAIVE: fixed-point source row
+    double* s_iM = reinterpret_cast<double*>(s_Y0 + 4 * ((it.oh + 4 * R + 3) / 4));  // [6] NAIVE: inverse affine map of the call
+
     if (NAIVE) {
         // the call's map: from its filterRect and its plane -- in the PatchMatch phase the step's proposal, which the block above
         // left in s_pl (read after its barrier), so every work item of a cell builds the same map from the same bits (DESIGN.md 3b)
@@ -490,7 +504,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
     }
 
     {   // zero-fill: the box filter is zero padded (GuidedFilter.h:43 BORDER_CONSTANT)
-        const int total = (K * VW + 1) / 2 + K * W2 + 8 * kCH * SW;
+        const int total = (K * VW + 1) / 2 + K * W2 + handoff_f4(VW, R);
         if (!PM) for (int i = tid; i < total; i += kThreads) smem[i] = f4zero();
         for (int v = tid; v < VHs; v += kThreads) {
             const int y = ys + v;
@@ -565,7 +579,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
                 }
                 produce_begin(0, c, kLinkAH);
                 if (t < VW) {
-                    F4* hb = hb1 + (c & 1) * kCH * SW + sidx(t);
+                    F4* hb = hb1 + (c & 1) * kCH * SW1 + sidx(t);
 #pragma unroll
                     for (int r = 0; r < kCH; r++) {
                         uint2* sl = ring1 + slot * VW + t;
@@ -577,7 +591,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
                         const float o1 = fmaf(__uint_as_float(__byte_perm(oldpg.y, 0x4B000000u, 0x7441)), pso, nmo);
                         const float o2 = fmaf(__uint_as_float(__byte_perm(oldpg.y, 0x4B000000u, 0x7442)), pso, nmo);
                         acc = f4add(acc, f4sub(nwr[r], F4{pk2(po, o0), pk2(o1, o2)}));
-                        hb[r * SW] = acc;
+                        hb[r * SW1] = acc;
                         slot = (slot + 1 == K) ? 0 : slot + 1;
                     }
                 }
@@ -607,11 +621,12 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
         const float maxd = (float)(P.D - 1);
         F4 acc = f4zero();
         int slot = 0;
-        // Gather batches of kG rows.  Exactly ONE batch of loads is in flight at any time: the hardware
+        constexpr int G = MIN_CTAS == kLeanCtas ? 4 : kG;
+        // Gather batches of G rows.  Exactly ONE batch of loads is in flight at any time: the hardware
         // scoreboard cannot tell older from younger loads, so a deeper register pipeline would stall on the
         // youngest load.  Order per batch: wait(batch b) -> issue(batch b+1) -> process(batch b).
-        float lv0[kG], lv1[kG], lf1[kG];
-        uint32_t lg[kG];
+        float lv0[G], lv1[G], lf1[G];
+        uint32_t lg[G];
         // weight f1 and slice indices for plane disparity d
         //   fast: d < 0 -> V[0]; d >= D-1 -> (1-1) V[D-2] + 1 V[D-1] = V[D-1]; else lerp (:78-92)
         //   generic: f1 in [0,1] lerp | 2: COST_FOR_INVALID | 3: C = V[d0] | -1: outside filterRect
@@ -639,7 +654,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
         int vi = 0;  // next virtual row to issue
         auto issue = [&]() {
 #pragma unroll
-            for (int j = 0; j < kG; j++) {
+            for (int j = 0; j < G; j++) {
                 lv0[j] = 0.f; lv1[j] = 0.f; lg[j] = 0u; lf1[j] = fast ? 0.f : -1.f;  // outside filterRect: zero
                 if (colA && vi < vReal) {
                     int d0, d1;
@@ -665,11 +680,11 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
         issue();
         int c = 0;  // pipeline chunk
         while (c < nChunks) {
-            LEXP_TRACE_LOAD_WAIT(lg[kG - 1]);  // the youngest load of the batch in flight
-            float wp[kG];
-            uint32_t wg[kG];
+            LEXP_TRACE_LOAD_WAIT(lg[G - 1]);  // the youngest load of the batch in flight
+            float wp[G];
+            uint32_t wg[G];
 #pragma unroll
-            for (int j = 0; j < kG; j++) {
+            for (int j = 0; j < G; j++) {
                 // consume point of the batch: every load must have landed before the next batch is issued
                 LEXP_LOADS_LANDED("+f"(lv0[j]), "+f"(lv1[j]), "+r"(lg[j]));
                 const float f1 = lf1[j];
@@ -685,11 +700,11 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
             }
             issue();
 #pragma unroll
-            for (int cc = 0; cc < kG / kCH; cc++) {
+            for (int cc = 0; cc < G / kCH; cc++) {
                 if (c < nChunks) {  // CTA-uniform
                     produce_begin(0, c, kLinkAH);
                     if (t < VW) {
-                        F4* hb = hb1 + (c & 1) * kCH * SW + sidx(t);
+                        F4* hb = hb1 + (c & 1) * kCH * SW1 + sidx(t);
 #pragma unroll
                         for (int r = 0; r < kCH; r++) {
                             const int j = cc * kCH + r;
@@ -712,7 +727,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
                             const F4 nw = F4{pk2(p, q0), pk2(q1, q2)};
                             const F4 old = F4{pk2(po, o0), pk2(o1, o2)};
                             acc = f4add(acc, f4sub(nw, old));
-                            hb[r * SW] = acc;  // column sum centred on row y - R
+                            hb[r * SW1] = acc;  // column sum centred on row y - R
                             slot = (slot + 1 == K) ? 0 : slot + 1;
                         }
                     }
@@ -733,13 +748,14 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
         const int vmin = st2 ? vE0 : vC0, vmax = st2 ? VHs : vC1;
         const F4* inb = st2 ? hb2 : hb1;
         F4* outb = st2 ? ho2 : ho1;
+        const int sin = st2 ? SW2 : SW1, sout = st2 ? SWo : SW2;
         for (int c = 0; c < nChunks; c++) {
             const int v = c * kCH + r;
             consume_begin(lin, c, nin);
             produce_begin(lout, c, nout);
             if (k < nruns && v >= vmin && v < vmax) {
-                const F4* in = inb + ((c & 1) * kCH + r) * SW + 9 * k;
-                F4* out = outb + ((c & 1) * kCH + r) * SW + 9 * k;
+                const F4* in = inb + ((c & 1) * kCH + r) * sin + 9 * k;
+                F4* out = outb + ((c & 1) * kCH + r) * sout + 9 * k;
                 if (R_T > 0) {
                     F4 w[kRun - 1];
                     F4 s = in[0], s2 = in[1];  // two partial sums: halves the dependent add chain
@@ -780,7 +796,9 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
         if (colC) inv_nx = 1.0f / (float)(min(XC + R, fx1 - 1) - max(XC - R, it.fx) + 1);
         F4 acc = f4zero();
         int slot = 0;
-        // one batch (= one chunk) of statistics loads in flight: wait(c) -> issue(c + 1) -> process(c)
+        // one batch (= one chunk) of statistics loads in flight: wait(c) -> issue(c + 1) -> process(c).  The lean build issues
+        // row r of c + 1 right after processing row r of c instead: the batch then needs no second set of registers
+        constexpr bool kRowIssue = MIN_CTAS == kLeanCtas;
         float4 sa[kCH], sb[kCH];
         float sc[kCH];
         // statistics of centre row yc = ys + v - R, issued chunk by chunk in order
@@ -789,18 +807,19 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
         const float4* pa = P.statA + pix0;
         const float4* pb = P.statB + pix0;
         const float* pc = P.statC + pix0;
+        auto issue_row = [&](int r) {
+            sa[r] = make_float4(0.f, 0.f, 0.f, 0.f); sb[r] = sa[r]; sc[r] = 0.f;
+            if (colC && vi >= vC0 && vi < vC1) {
+                sa[r] = __ldg(pa);
+                sb[r] = __ldg(pb);
+                sc[r] = __ldg(pc);
+            }
+            vi++;
+            pa += P.W; pb += P.W; pc += P.W;
+        };
         auto issue = [&]() {
 #pragma unroll
-            for (int r = 0; r < kCH; r++) {
-                sa[r] = make_float4(0.f, 0.f, 0.f, 0.f); sb[r] = sa[r]; sc[r] = 0.f;
-                if (colC && vi >= vC0 && vi < vC1) {
-                    sa[r] = __ldg(pa);
-                    sb[r] = __ldg(pb);
-                    sc[r] = __ldg(pc);
-                }
-                vi++;
-                pa += P.W; pb += P.W; pc += P.W;
-            }
+            for (int r = 0; r < kCH; r++) issue_row(r);
         };
         issue();
         for (int c = 0; c < nChunks; c++) {
@@ -814,12 +833,12 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
                                       "+f"(sb[r].z), "+f"(sb[r].w), "+f"(sc[r]));
                     ca[r] = sa[r]; cb[r] = sb[r]; cc[r] = sc[r];
                 }
-                issue();
+                if (!kRowIssue) issue();
                 consume_begin(1, c, kLinkHC);
                 produce_begin(2, c, kLinkCH);
                 if (t < W2) {
-                    const F4* ho = ho1 + (c & 1) * kCH * SW + sidx(t);
-                    F4* hb = hb2 + (c & 1) * kCH * SW + sidx(t);
+                    const F4* ho = ho1 + (c & 1) * kCH * SW2 + sidx(t);
+                    F4* hb = hb2 + (c & 1) * kCH * SW2 + sidx(t);
 #pragma unroll
                     for (int r = 0; r < kCH; r++) {
                         const int v = c * kCH + r;
@@ -827,7 +846,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
                             F4 ab = f4zero();
                             if (colC && v < vC1) {
                                 const float invN = inv_nx * s_invny[v - R];
-                                const F4 B = ho[r * SW];
+                                const F4 B = ho[r * SW2];
                                 float Bp, B0, B1, B2;
                                 up2(B.lo, Bp, B0); up2(B.hi, B1, B2);
                                 const float m0 = ca[r].x, m1 = ca[r].y, m2 = ca[r].z, i00 = ca[r].w;
@@ -846,9 +865,10 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
                             const F4 old = *sl;
                             *sl = ab;
                             acc = f4add(acc, f4sub(ab, old));
-                            hb[r * SW] = acc;  // column sum centred on row y - 2R
+                            hb[r * SW2] = acc;  // column sum centred on row y - 2R
                             slot = (slot + 1 == K) ? 0 : slot + 1;
                         }
+                        if (kRowIssue) issue_row(r);   // columns t >= W2 never load (colC is false there)
                     }
                 }
                 consume_end(1, c, nChunks, kLinkHC);
@@ -878,22 +898,25 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
             const float margin = 1e-5f * mag + 1e-30f;
             if (axl + byl + pl.c - ext - margin >= P.min_disp && axh + byh + pl.c + ext + margin <= P.max_disp) check = false;
         }
+        // one batch (= one chunk) of guide (and current-cost) loads in flight, issued like team C's
+        constexpr bool kRowIssue = MIN_CTAS == kLeanCtas;
         uint32_t gq[kCH];
         float cq[kCH];   // PatchMatch phase: the pixel's current cost, prefetched with the guide (L2 only: other SMs wrote it)
         const bool pm_update = PM && P.pm_mode == 1;
         int vi = 0;
         const unsigned int* pg = reinterpret_cast<const unsigned int*>(P.guide) + (size_t)(ys - 2 * R) * P.W + (colE ? XE : it.ox0);
+        auto issue_row = [&](int r) {
+            gq[r] = 0u; cq[r] = 0.f;
+            if (colE && vi >= vE0 && vi < VHs) {
+                gq[r] = __ldg(pg);
+                if (pm_update) cq[r] = __ldcg(P.cur_cost + (pg - reinterpret_cast<const unsigned int*>(P.guide)));
+            }
+            vi++;
+            pg += P.W;
+        };
         auto issue = [&]() {
 #pragma unroll
-            for (int r = 0; r < kCH; r++) {
-                gq[r] = 0u; cq[r] = 0.f;
-                if (colE && vi >= vE0 && vi < VHs) {
-                    gq[r] = __ldg(pg);
-                    if (pm_update) cq[r] = __ldcg(P.cur_cost + (pg - reinterpret_cast<const unsigned int*>(P.guide)));
-                }
-                vi++;
-                pg += P.W;
-            }
+            for (int r = 0; r < kCH; r++) issue_row(r);
         };
         issue();
         size_t cpix = (size_t)it.oy0 * P.W + XE;   // PatchMatch phase: pixel index of the next output row in cur_cost / cur_label
@@ -912,15 +935,15 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
                     LEXP_LOADS_LANDED("+r"(gq[r]), "+f"(cq[r]));
                     cg[r] = gq[r]; cc[r] = cq[r];
                 }
-                issue();
+                if (!kRowIssue) issue();
                 consume_begin(3, c, kLinkHE);
                 if (colE) {
-                    const F4* ho = ho2 + (c & 1) * kCH * SW + sidx(t);
+                    const F4* ho = ho2 + (c & 1) * kCH * SWo + sidx(t);
 #pragma unroll
                     for (int r = 0; r < kCH; r++) {
                         const int v = c * kCH + r;
                         if (v >= vE0 && v < VHs) {
-                            const F4 S = ho[r * SW];
+                            const F4 S = ho[r * SWo];
                             float S0, S1, S2, Sb;
                             up2(S.lo, S0, S1); up2(S.hi, S2, Sb);
                             const uint32_t g = cg[r];
@@ -965,6 +988,7 @@ __global__ void __launch_bounds__(kThreads, kMinCtas) lexp_fused_kernel(const KP
                                 orow += ostride;
                             }
                         }
+                        if (kRowIssue) issue_row(r);   // columns t >= ow never load (colE is false there)
                     }
                 }
                 consume_end(3, c, nChunks, kLinkHE);

@@ -170,6 +170,12 @@ LEXP_API int64_t lexp_launch_count(const lexp_ctx* ctx);
 /* how many of this context's launches of lexp_fused_kernel carried the programmatic-serialization attribute, i.e. may have
  * overlapped the launch before them (0 when LEXP_PDL_OFF=1 was set at lexp_create). */
 LEXP_API int64_t lexp_overlapped_launch_count(const lexp_ctx* ctx);
+/* how many of this context's launches of lexp_fused_kernel ran its lean build: the cost-volume PatchMatch-phase kernel at windR 20 / 21
+ * compiled for three resident CTAs per SM instead of two (DESIGN.md 3a).  By default a launch takes it when it has more work items than
+ * 2 x #SM and three of its widest item fit in an SM's shared memory.  LEXP_LEAN in the environment at lexp_create overrides that rule:
+ * LEXP_LEAN=0 never takes the lean build, LEXP_LEAN=1 takes it for every such launch whatever its size.  Planning does not depend on
+ * the setting, and both builds compute the same outputs bit for bit; it exists to test the one build against the other. */
+LEXP_API int64_t lexp_lean_launch_count(const lexp_ctx* ctx);
 /* Concurrent lexp_eval_cell calls (the OpenMP loop of FastGCStereo.h:30-49, one blocking call per cell and thread) are
  * combined: calls that arrive while the device is busy are evaluated together in one batched launch.  Returns how many
  * such launches there were and how many calls they served (calls that found the device idle are not counted).

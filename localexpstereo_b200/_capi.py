@@ -61,6 +61,7 @@ SYMBOLS = {
     "lexp_set_overlap": (C.c_int, [_P, C.c_int]),
     "lexp_launch_count": (C.c_int64, [_P]),
     "lexp_overlapped_launch_count": (C.c_int64, [_P]),
+    "lexp_lean_launch_count": (C.c_int64, [_P]),
     "lexp_combine_stats": (C.c_int, [_P, C.POINTER(C.c_int64), C.POINTER(C.c_int64)]),
     "lexp_pm_begin": (C.c_int, [_P, C.c_int, _P, _P]),
     "lexp_pm_get": (C.c_int, [_P, C.c_int, _P, _P]),

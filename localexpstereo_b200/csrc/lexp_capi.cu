@@ -143,6 +143,8 @@ struct lexp_ctx {
     float* d_ransac_disp = nullptr;                // LEXP_PROP_RANSAC: float[H][W], the disparities of the snapshot of every cell's unitRegion
     int64_t launches = 0;
     int64_t overlapped_launches = 0;   // fused launches that carried the programmatic-serialization attribute
+    int64_t lean_launches = 0;         // fused launches of the lean build (kLeanCtas)
+    int lean = -1;                     // LEXP_LEAN: -1 unset (launch_fused's rule), 0 never the lean build, 1 every launch that has one
     std::mutex mu;
     int tile_oh = 128;    // max output rows per work item
     bool tile_oh_fixed = false;  // LEXP_TILE_OH given: no per-plan search
@@ -318,6 +320,7 @@ int launch_fused_t(lexp_ctx* c, const KParams& kp_in, int nitems, size_t smem, b
     LEXP_LAUNCH(kern, nitems, kThreads, smem, c->stream, kp);
     LEXP_CUDA(cudaGetLastError());
     c->launches++;
+    if (MIN_CTAS == kLeanCtas) c->lean_launches++;
     c->chain_ok = true;
 #if LEXP_TRACE
     report_trace(c, nitems);
@@ -343,8 +346,9 @@ int launch_fused(lexp_ctx* c, const KParams& kp, int nitems, size_t smem, bool a
         // R = 10: the lean build (3 CTAs per SM) when three of the launch's widest item fit in shared memory and the launch has more
         // items than kMinCtas x #SM slots.  A launch that fits in those slots gains no warps from it, only fewer loads in flight per
         // CTA (measured: a 240-item layer-2 launch of the 2048x1536 sweep ran 25 % slower lean).  Unary-cost launches keep the kMinCtas
-        // build: the lean one made bench.py's unary sweep 21 % slower.
-        const bool lean = fused_fits_lean(smem) && (int64_t)nitems > (int64_t)kMinCtas * c->num_sms;
+        // build: the lean one made bench.py's unary sweep 21 % slower.  LEXP_LEAN=0 / 1 overrides the rule (the outputs are the same;
+        // a lean launch of an item over fused_fits_lean's limit simply has fewer CTAs resident).
+        const bool lean = c->lean >= 0 ? c->lean == 1 : fused_fits_lean(smem) && (int64_t)nitems > (int64_t)kMinCtas * c->num_sms;
         switch (c->R) {
             case 10: return lean ? launch_fused_t<10, false, true, kLeanCtas>(c, kp, nitems, smem, allow_pdl)
                                  : launch_fused_t<10, false, true>(c, kp, nitems, smem, allow_pdl);
@@ -648,6 +652,7 @@ int lexp_create(const lexp_params* params, lexp_ctx** out_ctx) {
     // default build (2 CTAs) no cap is needed at R = 10: the widest tile needs ~76 KB (at R = 16 it needs ~117 KB: one CTA per SM).
     c->ctas_per_sm = env_int("LEXP_CTAS_PER_SM", kMinCtas);
     c->pdl = !env_int("LEXP_PDL_OFF", 0);
+    c->lean = getenv("LEXP_LEAN") && *getenv("LEXP_LEAN") ? (env_int("LEXP_LEAN", 0) != 0) : -1;
     c->combine = env_int("LEXP_COMBINE", 1) != 0;
     c->comb_window_us = std::max(0, env_int("LEXP_COMBINE_WINDOW_US", 30));
     c->smem_cap = (size_t)env_int("LEXP_SMEM_CAP", 0);
@@ -1278,6 +1283,7 @@ int lexp_set_stream(lexp_ctx* c, void* s) {
 }
 int64_t lexp_launch_count(const lexp_ctx* c) { return c ? c->launches : 0; }
 int64_t lexp_overlapped_launch_count(const lexp_ctx* c) { return c ? c->overlapped_launches : 0; }
+int64_t lexp_lean_launch_count(const lexp_ctx* c) { return c ? c->lean_launches : 0; }
 
 int lexp_set_overlap(lexp_ctx* c, int on) {
     if (!c) return fail(LEXP_ERR_INVALID, "null ctx");

@@ -463,6 +463,11 @@ class CostVolumeEnergy:
         return int(lib().lexp_overlapped_launch_count(self._h))
 
     @property
+    def lean_launch_count(self) -> int:
+        """How many of launch_count ran the lean (three CTAs per SM) build of the PatchMatch-phase kernel: see lexp_lean_launch_count."""
+        return int(lib().lexp_lean_launch_count(self._h))
+
+    @property
     def combine_stats(self):
         """(batched launches that served concurrent single-cell calls, number of calls they served)."""
         b, n = C.c_int64(0), C.c_int64(0)

@@ -203,9 +203,16 @@ LEXP_API int lexp_combine_stats(const lexp_ctx* ctx, int64_t* batches, int64_t* 
                                   of a context allocates an H x W float scratch: issue it before capturing a CUDA graph */
 #define LEXP_PM_INIT 1         /* flags: unconditional write of cost and label (initCurrentFast, FastGCStereo.h:105-113) */
 /* (Re)start the state of view `mode`: currentCost = cost (NULL: +INFINITY, FastGCStereo.h:137), currentLabeling = labeling
- * (NULL: zeros); host arrays float[H][W] / lexp_plane[H][W]. */
+ * (NULL: zeros); host arrays float[H][W] / lexp_plane[H][W].  On a view not connected to peers it also clears the error that a
+ * graph-cut move which stopped at its round limit left (lexp_pm_get); a timed-out wait for a group epoch is not cleared.  Blocking
+ * whenever the view already has a state (it reads the error word back) or a host array is given; not for use inside a CUDA graph
+ * capture. */
 LEXP_API int lexp_pm_begin(lexp_ctx* ctx, int mode, const float* cost_host, const lexp_plane* labeling_host);
-/* Copy the state back (either pointer may be NULL); blocking. */
+/* Copy the state back (either pointer may be NULL); blocking.  The state is copied in any case; the return value is then
+ * LEXP_ERR_STATE if a graph-cut move of this view stopped at its round limit (the state is not the result of minimum cuts: every
+ * pixel of the move's cells holds its old state or the proposal; cleared by the next lexp_pm_begin of a view not connected to peers)
+ * or if a wait for a group epoch timed out (the state is incomplete; sticky for the life of the context).  The round limit is 2^22
+ * push / relabel rounds per move; the environment variable LEXP_GC_MAX_ROUNDS, read by lexp_create, overrides it (a test hook). */
 LEXP_API int lexp_pm_get(lexp_ctx* ctx, int mode, float* cost_host, lexp_plane* labeling_host);
 /* Device pointers of the state (for callers that keep working on the device: multi-GPU exchange, disparity maps). */
 LEXP_API int lexp_pm_device_state(lexp_ctx* ctx, int mode, float** d_cost, lexp_plane** d_labeling);

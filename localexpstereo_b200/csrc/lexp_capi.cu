@@ -659,6 +659,7 @@ int lexp_create(const lexp_params* params, lexp_ctx** out_ctx) {
     c->gc_threads = std::min(1024, std::max(32, env_int("LEXP_GC_THREADS", 1024) / 32 * 32));
     c->gc_relabel_every = std::max(1, env_int("LEXP_GC_RELABEL_EVERY", 24));
     c->gc_big_nodes = std::max(0, env_int("LEXP_GC_BIG_NODES", 32768));
+    c->gc_max_rounds = std::max(0, env_int("LEXP_GC_MAX_ROUNDS", 1 << 22));   // test hook: the round limit of a move
     c->upload_slab_mb = env_int("LEXP_UPLOAD_SLAB_MB", 512);
 #if LEXP_TRACE
     if (const char* path = getenv("LEXP_TRACE_FILE")) c->trace_file = path;
@@ -1302,6 +1303,12 @@ int lexp_pm_begin(lexp_ctx* c, int mode, const float* cost, const lexp_plane* la
     if (!c->d_flags[mode]) {
         LEXP_CUDA(cudaMalloc(&c->d_flags[mode], (kMaxPeers + 2) * sizeof(int)));   // + epoch base + error flag
         LEXP_CUDA(memset0(c, c->d_flags[mode], (kMaxPeers + 2) * sizeof(int)));   // epochs only grow: never reset while peers run
+    } else if (c->peers[mode].world <= 1) {
+        // a move that stopped at its round limit (2) concerns the state this call replaces; a peer timeout (1) stays
+        int err = 0;
+        LEXP_CUDA(d2h(c, &err, c->d_flags[mode] + kMaxPeers + 1, sizeof(int)));
+        LEXP_CUDA(cudaStreamSynchronize(c->stream));
+        if (err == 2) LEXP_CUDA(memset0(c, c->d_flags[mode] + kMaxPeers + 1, sizeof(int)));
     }
     if (cost) LEXP_CUDA(h2d(c, c->d_cur_cost[mode], cost, HW * sizeof(float)));
     else LEXP_CUDA(launch_aux(c, lexp_fill_f32, c->num_sms * 4, 256, c->d_cur_cost[mode], HW, __builtin_inff()));   // currentCost_ = INFINITY (:137)

@@ -8,6 +8,7 @@ stream, is compared with the recorded plane; check_pm_result / check_gc_result t
 Moves (certify_gc_step): one graph-cut step of a plan against the exact minimum cut of the same graph, move by move (the criteria are
 stated in tests/test_gpu_zz_gc_moves.py)."""
 import math
+import time
 
 import numpy as np
 
@@ -197,28 +198,44 @@ def proposal_costs(E, plan, planes, mode, devmem):
     return np.array(devmem.download(d), np.float32)
 
 
-def certify_gc_step(E, plan, regions, mode, lam, th, devmem, planes=None, kind=0, m=0, seed=0, exact=False, ties_ok=False):
+def certify_gc_step(E, plan, regions, mode, lam, th, devmem, planes=None, kind=0, m=0, seed=0, exact=False, ties_ok=False, coeff=None,
+                    state=None):
     """One proposal step of `plan` (Plan.gc_step: PROP_LIST with `planes`, or a device proposer) checked move by move, (a) to (d) of
     tests/test_gpu_zz_gc_moves.py.  Returns one record per cell.
     Tolerance of (b) to (d): 1e-6 * max(mf, 1e-3).  (b) also allows the double rounding of konst (the device sums it per thread and per
     block, the oracle per node and pairwise): 2 N u * (|konst| + mf + 8 N lam th) bounds any summation order of N terms whose
-    absolute values add up to at most that (a node's konst terms are >= -4 lam th).  exact: no tolerance at all."""
+    absolute values add up to at most that (a node's konst terms are >= -4 lam th).  exact: no tolerance at all.
+    coeff: the view's coefficient maps (E.smooth_coeff(mode)) when the caller already holds them (downloaded on every call otherwise).
+    state: a dict carrying the device state from one step to the next: its "cost" / "label" are taken as the pre-move state when
+    present (downloaded otherwise), and the post-move state is stored there, with "step_s" (wall time of the step up to its
+    synchronisation) and "phase" (whether the phase kernels ran it: a one-CTA step is the unary launches of the plan plus at most a
+    proposal launch and the move kernel, a phase step issues at least one launch per phase)."""
     import localexpstereo_b200 as L
     H, W = E.height, E.width
     n = len(regions)
     assert_non_adjacent(regions)
     assert (kind == L.PROP_LIST) == (planes is not None)
-    pre_c, pre_l = E.pm_get(mode)
-    coeff = E.smooth_coeff(mode)
+    if state is not None and "cost" in state:
+        pre_c, pre_l = state["cost"], state["label"]
+    else:
+        pre_c, pre_l = E.pm_get(mode)
+    if coeff is None:
+        coeff = E.smooth_coeff(mode)
     d_pl, d_fl = devmem.zeros((n, 4)), devmem.zeros((n, 2))
+    E.sync()
+    n0, t0 = E.launch_count, time.perf_counter()
     plan.gc_step(kind, m, seed, planes=planes, d_planes_out=devmem.ptr(d_pl), d_flows_out=devmem.ptr(d_fl), mode=mode)
     E.sync()
+    step_s, n_step = time.perf_counter() - t0, E.launch_count - n0
     post_c, post_l = E.pm_get(mode)
     used = np.array(devmem.download(d_pl), np.float32)
     flows = np.ascontiguousarray(devmem.download(d_fl)).view(np.float64)[:, 0].copy()
     if planes is not None:
         assert np.array_equal(bits(used), bits(np.reshape(planes, (n, 4))))
+    n0 = E.launch_count
     q_img = proposal_costs(E, plan, used, mode, devmem)
+    if state is not None:
+        state.update(cost=post_c, label=post_l, step_s=step_s, phase=n_step - (E.launch_count - n0) > 2)
     inside = np.zeros((H, W), bool)
     cells = []
     for i, reg in enumerate(regions):

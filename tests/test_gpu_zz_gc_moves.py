@@ -148,10 +148,8 @@ def corridor(w, h):
         y += w - 3
 
 
-def scene_corridor(devmem, w=40, h=800, mode=0):
-    """Two cells, each one corridor between zero-capacity walls (walls: sink capacity 64, no excess), arcs of 6 along it.  Cell A: excess 8
-    at the start, sink capacity 5 at the end -- maximum flow 5, unique minimum cut: the whole corridor takes the proposal.  Cell B: 5 and 8
-    -- maximum flow 5 again, unique minimum cut: the corridor keeps its labels.  Both flows travel the whole path."""
+def corridor_scene(w, h):
+    """(guide, regions, tr, labels, path) of scene_corridor."""
     H, W = h + 2, 2 * w + 3
     regions = [(1, 1, w, h), (w + 2, 1, w, h)]
     path = corridor(w, h)
@@ -163,9 +161,17 @@ def scene_corridor(devmem, w=40, h=800, mode=0):
             tr[ry + y, rx + x] = 0.0
         tr[ry + path[0][1], rx + path[0][0]] = a
         tr[ry + path[-1][1], rx + path[-1][0]] = b
+    return guide, regions, tr, level_labels(np.full((H, W), 3.0, np.float32)), path
+
+
+def scene_corridor(devmem, w=40, h=800, mode=0):
+    """Two cells, each one corridor between zero-capacity walls (walls: sink capacity 64, no excess), arcs of 6 along it.  Cell A: excess 8
+    at the start, sink capacity 5 at the end -- maximum flow 5, unique minimum cut: the whole corridor takes the proposal.  Cell B: 5 and 8
+    -- maximum flow 5 again, unique minimum cut: the corridor keeps its labels.  Both flows travel the whole path."""
+    guide, regions, tr, labels, path = corridor_scene(w, h)
     E = make_energy(guide, seed=2)
     try:
-        cells = run_designed(E, regions, tr, level_labels(np.full((H, W), 3.0, np.float32)), mode, devmem)
+        cells = run_designed(E, regions, tr, labels, mode, devmem)
         on = np.zeros((h, w), bool)
         on[tuple(np.array(path).T[::-1])] = True
         assert np.array_equal(cells[0]["mask"], on), "the corridor of cell A must take the proposal, its walls must not"

@@ -660,7 +660,11 @@ def pm_rng_state(seed, cell_id):
 
 
 def pm_proposal(kind, m, state, cur_label, unit, min_disp, max_disp):
-    """kind 1: ExpansionProposer::getNextProposal (Proposer.h:69-75); kind 2: RandomProposer::getNextProposal (:120-148)."""
+    """kind 1: ExpansionProposer::getNextProposal (Proposer.h:69-75); kind 2: RandomProposer::getNextProposal (:120-148);
+    kind 3: RansacProposer(1) (:155-312, oracle/ransac_oracle.py)."""
+    if kind == 3:
+        from .ransac_oracle import ransac_proposal   # it imports this module for CvRNG
+        return ransac_proposal(state, cur_label, unit)[0]
     rng = CvRNG(state)
     ux, uy, uw, uh = unit
     n = rng.uniform_int(0, uw * uh)                 # selectRandomPixelInRect (:38-45)

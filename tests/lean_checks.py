@@ -8,13 +8,13 @@ launches of more than 2 x #SM work items whose widest item leaves room for three
 R = 10 cost-volume PatchMatch-phase launch and LEXP_LEAN=0 forbids it, without changing the plans.  So:
   check A: contexts under LEXP_LEAN=1, =0 and unset run the same steps on the same inputs; after every step (designed scenes) or
            every group (sweeps) currentCost, currentLabeling and the recorded planes must be bit-identical;
-  check B: test_gpu_zz_pm_steps.Rig with both contexts under LEXP_LEAN=1: every step certified -- the update rule bit for bit, the lean
+  check B: pm_step_rig.Rig with both contexts under LEXP_LEAN=1: every step certified -- the update rule bit for bit, the lean
            q against the FP64 oracle, and the lean PatchMatch q against the two-CTA unary instantiation bit for bit.
 Every check asserts from lexp_lean_launch_count that the build it means to test ran."""
 import numpy as np
 
 from lexp_testlib import bits, make_scene, seeded_labels
-from test_gpu_zz_pm_steps import Rig, Tally, assert_same_state, run_sweep  # noqa: F401
+from pm_step_rig import Rig, assert_same_state, run_sweep
 
 R10 = 10          # windR 20 and 21: the radius the lean build exists for
 OW_MAX = 64       # max_tile_ow(10): the planner's widest column tile
@@ -355,7 +355,7 @@ def compare_walks(devmem, sweeps, labels, iterations, seed, on_layer_end=None):
 
 
 def sweep_certified(devmem, monkeypatch, sc, iterations=1):
-    """Check B on a sweep: test_gpu_zz_pm_steps.run_sweep with both contexts under LEXP_LEAN=1."""
+    """Check B on a sweep: pm_step_rig.run_sweep with both contexts under LEXP_LEAN=1."""
     monkeypatch.setenv("LEXP_TILE_OH", str(sc.tile_oh))
     imL, imR, volL, volR = sc.scene()
     R = under_lean(monkeypatch, 1, lambda: Rig(devmem, imL, imR, volL, volR, sc.windR, sc.units, sc.proposers, sc.mode, sc.MIN, sc.MAX))

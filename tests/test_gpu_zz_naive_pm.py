@@ -1,9 +1,9 @@
 """The PatchMatch phase of the image-based energy (NaiveStereoEnergy, BASELINE.json configs[0] `-mode MiddV2`: initCurrentFast, two pm
 iterations, then the graph-cut iterations, main.cpp:21,310-312) on the device.
 
-Per-step certification (tests/naive_pm_checks.py: proposals, update rule, PatchMatch = unary instantiation, oracle costs) on the
-cones crop with the reference's proposer lists, at a generic radius, with v != 0 and at 2048 x 1536; the MiddV2-shaped run with the
-Python and the native schedule; the launch paths; the refusal on a connected cell shard.
+Per-step certification (tests/pm_step_rig.py on the scenes of tests/naive_pm_checks.py: proposals, update rule, PatchMatch = unary
+instantiation, oracle costs) on the cones crop with the reference's proposer lists, at a generic radius, with v != 0 and at
+2048 x 1536; the MiddV2-shaped run with the Python and the native schedule; the launch paths; the refusal on a connected cell shard.
 (Sorted after the graph-cut tests and before the large-size tests.)"""
 import time
 
@@ -188,7 +188,7 @@ def test_naive_pm_iteration_at_2048x1536():
     W, H, D = 2048, 1536, 256
     imL, imR = synth.synthetic_image(H, W, 42), synth.synthetic_image(H, W, 43)
     dm = TorchDeviceMemory()
-    R = NP.NaiveRig(dm, imL, imR, D, 20, NP.MIDDV2_UNITS, NP.reference_lists(3), q_cells=3, seed=4)
+    R = NP.naive_rig(dm, imL, imR, D, 20, NP.MIDDV2_UNITS, NP.reference_lists(3), q_cells=3, seed=4)
     try:
         last = {}
         for (li, gi, g, _) in R.S.schedule:
@@ -198,7 +198,7 @@ def test_naive_pm_iteration_at_2048x1536():
         R.Sq.begin()
         R.S.begin()
         R.S.init(labels)
-        n = R.iteration(0, 4321, certify=lambda g: g.group in (0, last[g.layer]))
+        n, _ = R.iteration(0, 4321, certify=lambda g: g.group in (0, last[g.layer]))
         c, l = R.S.get()
         assert np.isfinite(c).all()
         print(R.T.line("2048 x 1536 x 256") + f"; {n} launches, {time.perf_counter() - t0:.1f} s in all")

@@ -1,32 +1,17 @@
-"""Every PatchMatch step of the device against the oracle's update of the SAME state.
-
-tests/test_gpu_pm.py replays the device's planes in the numpy oracle on the oracle's own state, which drifts from the device's at
-FP32 / FP64 cost ties, so it needs budgets.  Here every step starts from the device's own pre-step state (pm_get) and is certified
-without a budget (Rig.certify):
-  (P) proposal: the oracle's proposer (oracle.pm_proposal) on the device's pre-step labeling, with the launch's random stream, gives
-      the plane the step recorded -- bit for bit for lists and ExpansionProposer; RandomProposer within 2e-6 relative / 1e-6 absolute
-      (CUDA's FP64 sin / cos against glibc's), its fourth component bit for bit;
-  (U) update: nothing outside the group's targetRects changes; inside, post = (pre_cost > q) ? (q, plane) : pre bit for bit (a NaN
-      cost never updates), or (q, plane) unconditionally for an initialisation.  q is the PatchMatch instantiation's own proposal
-      cost: the recorded planes run as an initialisation on a twin context (same inputs, its own state and schedule);
-  (Q) q against the FP64 C oracle (oracle.c_oracle, which tests/test_ref_pin.py pins to the reference): 1e-4 relative, the exact
-      COST_FOR_INVALID mask and the NaN pattern;
-  (I) q equals the unary instantiation's cost of the same planes (Plan.eval_device: image output, with the check) bit for bit --
-      the graph-cut steps take their proposal costs from that instantiation.
-Steps are issued one at a time with a synchronisation in between; the final state must equal the twin's uninterrupted sweep bit
-for bit (tests/test_gpu_launch_chains.py shows that overlapped launches equal serialized ones).
-
-Pixel tags: the fourth plane component v enters the cost only as 0 * v and through isfinite, and RandomProposer copies it.  With
-v = y * W + x in every pixel after the initialisation, a proposal names the pixel it was drawn from.
+"""Every PatchMatch step of the cost-volume energy on the device against the oracle's update of the SAME state: tests/pm_step_rig.py
+certifies each step without a budget -- (P) the proposal, (U) the update rule bit for bit, (Q) the proposal cost against the FP64 C
+oracle on every target pixel, (I) the PatchMatch cost equals the unary instantiation's -- and the states carry pixel tags, so every
+proposal names the pixel it was drawn from.  Designed scenes (ragged units, the update rule at its edges, MIN / MAX that take the
+generic sampler, many work items per cell, RandomProposer at the ends of m), the benchmark's workload layer by layer and two sizes.
 (Sorted after the graph-cut tests and before the large-size tests.)"""
 import time
 
 import numpy as np
 import pytest
 
-from oracle import c_oracle
 from oracle import lexp_oracle as O
-from lexp_testlib import TorchDeviceMemory, assert_costs_close, bits, make_scene, seeded_labels
+from lexp_testlib import TorchDeviceMemory, bits, make_scene, seeded_labels
+from pm_step_rig import Rig, Tally, assert_same_state, run_sweep
 
 pytestmark = pytest.mark.gpu
 
@@ -36,252 +21,6 @@ INVALID = np.float32(O.COST_FOR_INVALID)
 @pytest.fixture(scope="module")
 def devmem():
     return TorchDeviceMemory()
-
-
-def ulps(a, b):
-    """Distance in units in the last place of two float32 arrays of the same sign."""
-    return np.abs(bits(a).astype(np.int64) - bits(b).astype(np.int64))
-
-
-class Tally:
-    def __init__(self):
-        self.steps = self.exact = self.n_exact = self.random = self.n_random = self.random_same = 0
-        self.named = self.n_named = 0
-        self.worst_q = 0.0
-        self.instantiations_agree = True
-        self.t_oracle = self.t_step = 0.0
-
-    def line(self, what):
-        frac = self.random_same / self.n_random if self.n_random else 1.0
-        return (f"{what}: {self.steps} steps certified; proposals: list / Expansion bit-identical {self.exact} of {self.n_exact}, "
-                f"Random within tolerance {self.random} of {self.n_random} ({frac:.4f} bit-identical); source pixels named by their tag "
-                f"{self.named} of {self.n_named}; worst q err vs the FP64 oracle {self.worst_q:.2e}; (I) PM = unary instantiation: "
-                f"{'held' if self.instantiations_agree else 'FAILED'}; {self.t_step:.1f} s certifying, {self.t_oracle:.1f} s of it in the C oracle")
-
-
-class Rig:
-    """The context under test E and its twin Eq on the same inputs, a PMSweep on each, the FP64 C oracle of the view and page-locked
-    buffers for the states."""
-
-    def __init__(self, devmem, imL, imR, volL, volR, windR, units, proposers, mode=0, MIN=0.0, MAX=None, vol_host=None):
-        import localexpstereo_b200 as L
-        from localexpstereo_b200.sweep import PMSweep
-        self.L, self.dm, self.mode = L, devmem, mode
-        vol = volR if mode else volL
-        D = int(vol.shape[0])
-        self.MAX = float(D - 1 if MAX is None else MAX)
-        self.MIN = float(MIN)
-        prm = L.Parameters(windR=windR, filterName="GF", filter_param1=1e-4, th_col=0.5)
-        self.E, self.Eq = [L.CostVolumeEnergy(imL, imR, volL, volR, prm, self.MAX, self.MIN) for _ in range(2)]
-        self.H, self.W = self.E.height, self.E.width
-        self.S, self.Sq = [PMSweep(E, unit_sizes=units, proposers=proposers, mode=mode) for E in (self.E, self.Eq)]
-        self.C = c_oracle.COracle(self.H, self.W, D, windR, 1e-4, 0.5, self.MAX, self.MIN)
-        self.C.set_image(mode, imR if mode else imL)
-        self.C.set_volume(mode, vol if vol_host is None else vol_host)
-        self.buf = {}
-        for k in ("pre", "post", "q"):
-            self.buf[k] = (np.empty((self.H, self.W), np.float32), np.empty((self.H, self.W, 4), np.float32))
-            for a in self.buf[k]:
-                L.host_register(a)
-        self.owner = {}
-        self.tags = (np.arange(self.H, dtype=np.float32)[:, None] * np.float32(self.W) + np.arange(self.W, dtype=np.float32)[None, :])
-        self.tagged = self.tag_check_pending = False
-        self.T = Tally()
-
-    def close(self):
-        for a in (x for pair in self.buf.values() for x in pair):
-            self.L.host_unregister(a)
-        for S in (self.S, self.Sq):
-            S.close()
-        for E in (self.E, self.Eq):
-            E.close()
-        self.C.close()
-
-    def get(self, E, key=None):
-        if key is None:
-            return E.pm_get(self.mode)
-        return E.pm_get(self.mode, out_cost=self.buf[key][0], out_labeling=self.buf[key][1])
-
-    def tag(self, E):
-        """v = y * W + x in every pixel of E's state (exact: below 2^24), the costs unchanged.  Tagging the state under test also
-        makes its next certified step check that the tags leave the proposal costs unchanged."""
-        assert self.H * self.W <= 1 << 24
-        c, l = self.get(E)
-        l[..., 3] = self.tags
-        E.pm_begin(self.mode, c, l)
-        if E is self.E:
-            self.tagged = self.tag_check_pending = True
-
-    def owner_of(self, targets):
-        """[H][W] int: the call whose targetRect holds the pixel, -1 outside all of them (they must be disjoint)."""
-        key = tuple(map(tuple, targets))
-        if key not in self.owner:
-            o = np.full((self.H, self.W), -1, np.int64)
-            for i, (x, y, w, h) in enumerate(targets):
-                assert (o[y:y + h, x:x + w] == -1).all(), "targetRects of one step overlap"
-                o[y:y + h, x:x + w] = i
-            self.owner[key] = o
-        return self.owner[key]
-
-    def twin_q(self, qplan, d_planes=None, planes=None):
-        """The PatchMatch instantiation's cost of the planes in every target pixel: an initialisation step on the twin."""
-        self.Eq.pm_reset_sync()
-        if d_planes is not None:
-            qplan.pm_step(0, self.L.PROP_LIST, planes=d_planes, planes_on_device=True, init=True, mode=self.mode)
-        else:
-            qplan.pm_step(0, self.L.PROP_LIST, planes=planes, init=True, mode=self.mode)
-        self.Eq.sync()
-        return self.get(self.Eq, "q")
-
-    def certify(self, g, qplan, kind, m=0, seed=0, step_index=0, init=False, planes=None, sync=None):
-        """One step of the GroupPlan g (qplan: the twin's plan of the same cells) checked by (P), (U), (Q) and (I) of the module docstring.
-        Returns (pre, post, inside, q): the states are views of buffers the next step overwrites; inside marks the target pixels,
-        q holds their proposal costs."""
-        L, E, dm, T = self.L, self.E, self.dm, self.T
-        t0 = time.perf_counter()
-        plan, units, targets, filters, ids = g.plan, g.units, g.targets, g.filters, g.ids
-        n = plan.num_calls
-        assert len(units) == n and (kind == L.PROP_LIST) == (planes is not None)
-        pre_c, pre_l = self.get(E, "pre")
-        rec = dm.zeros((n, 4), fill=np.nan)
-        plan.pm_step(step_index, kind, m, seed, planes=planes, d_planes_out=dm.ptr(rec), init=init, mode=self.mode, **(sync or {}))
-        E.sync()
-        post_c, post_l = self.get(E, "post")
-        used = np.array(dm.download(rec), np.float32)
-        # (P)
-        for i, u in enumerate(units):
-            if kind == L.PROP_LIST:
-                assert np.array_equal(bits(used[i]), bits(planes[i])), f"(P) call {i}: recorded {used[i]}, listed {planes[i]}"
-                T.n_exact += 1; T.exact += 1
-                continue
-            st = O.pm_rng_state(seed, ids[i])
-            mine = O.pm_proposal(kind, m, st, pre_l, u, self.MIN, self.MAX)
-            if self.tagged:
-                nn = O.CvRNG(st).uniform_int(0, u[2] * u[3])
-                sx, sy = u[0] + nn % u[2], u[1] + nn // u[2]
-                T.n_named += 1
-                T.named += int(pre_l[sy, sx, 3] == self.tags[sy, sx] and used[i, 3] == self.tags[sy, sx])
-            if kind == L.PROP_EXPANSION:
-                T.n_exact += 1
-                assert np.array_equal(bits(used[i]), bits(mine)), f"(P) Expansion, cell {ids[i]} unit {u}: device {used[i]}, oracle {mine}"
-                T.exact += 1
-            else:
-                T.n_random += 1
-                assert bits(used[i])[3] == bits(mine)[3] and np.allclose(used[i], mine, rtol=2e-6, atol=1e-6), \
-                    f"(P) Random m={m}, cell {ids[i]} unit {u}: device {used[i]!r}, oracle {mine!r}"
-                T.random += 1
-                T.random_same += int(np.array_equal(bits(used[i]), bits(mine)))
-        # q: the PatchMatch instantiation, on the twin
-        q_c, q_l = self.twin_q(qplan, d_planes=dm.ptr(rec))
-        own = self.owner_of(targets)
-        inside = own >= 0
-        plane_px = used[own[inside]]
-        q = q_c[inside]
-        assert np.array_equal(bits(q_l[inside]), bits(plane_px)), "the twin's initialisation did not write the recorded planes"
-        if self.tag_check_pending:   # v enters the cost as 0 * v only: the same planes with v = 0 cost the same, bit for bit
-            self.tag_check_pending = False
-            flat = used.copy()
-            flat[:, 3] = 0.0
-            q0 = self.twin_q(qplan, planes=flat)[0][inside]
-            assert np.array_equal(bits(q0), bits(q)), "pixel tags changed a proposal cost"
-        # (U)
-        pc, pl = pre_c[inside], pre_l[inside]
-        upd = np.ones(q.shape, bool) if init else pc > q
-        assert np.array_equal(bits(post_c[inside]), bits(np.where(upd, q, pc))), \
-            f"(U) cost: {int((bits(post_c[inside]) != bits(np.where(upd, q, pc))).sum())} target pixels differ from the rule"
-        assert np.array_equal(bits(post_l[inside]), bits(np.where(upd[:, None], plane_px, pl))), "(U) label differs from the rule"
-        assert np.array_equal(bits(post_c[~inside]), bits(pre_c[~inside])) and np.array_equal(bits(post_l[~inside]), bits(pre_l[~inside])), \
-            "(U) a pixel outside the step's targetRects changed"
-        # (Q)
-        t1 = time.perf_counter()
-        ref = np.zeros((self.H, self.W), np.float32)
-        self.C.unary_batch(self.mode, filters, targets, used, ref, with_check=True)
-        T.t_oracle += time.perf_counter() - t1
-        r = ref[inside]
-        nan = np.isnan(r)
-        assert np.array_equal(nan, np.isnan(q)), f"(Q) NaN pattern differs at {int((nan != np.isnan(q)).sum())} pixels"
-        T.worst_q = max(T.worst_q, assert_costs_close(q[~nan], r[~nan], f"(Q) step kind {kind} m {m}"))
-        # (I)
-        img = dm.zeros((self.H, self.W), fill=np.nan)
-        plan.eval_device(dm.ptr(rec), dm.ptr(img), self.W * 4, with_check=True, mode=self.mode, planes_on_device=True)
-        E.sync()
-        ev = np.array(dm.download(img), np.float32)[inside]
-        same = bits(ev) == bits(q)
-        if not same.all():
-            T.instantiations_agree = False
-            bad = ~same
-            raise AssertionError(f"(I) the PatchMatch and unary instantiations differ at {int(bad.sum())} of {bad.size} pixels, up to "
-                                 f"{int(ulps(ev[bad], q[bad]).max())} ulps (e.g. {ev[bad][0]!r} vs {q[bad][0]!r})")
-        T.steps += 1
-        T.t_step += time.perf_counter() - t0
-        return (pre_c, pre_l), (post_c, post_l), inside, q
-
-    # ---- the sweep's own walk (PMSweep.init / iteration_by_group), one step at a time ----------------------------------------------
-    def init(self, labels, certify=True):
-        def issue(g, steps):
-            ((k, kind, _, _, sync),) = steps
-            if certify:
-                self.certify(g, self.Sq.init_plan, kind, planes=np.asarray(labels, np.float32), init=True, sync=sync)
-            else:
-                g.plan.pm_step(k, kind, planes=labels, init=True, mode=self.mode, **sync)
-        for _ in self.S.walk(None, 0, issue):
-            pass
-
-    def iteration(self, it, seed, certify=lambda li: True, snap_layer=None):
-        """One iteration of the sweep under test; steps of the layers `certify` selects are certified.  Returns the state at the end
-        of layer snap_layer (None: not taken)."""
-        S, snap = self.S, None
-        twin = {(g.layer, g.group): g.plan for g in self.Sq.groups}
-
-        def issue(g, steps):
-            for k, kind, m, sd, sync in steps:
-                if certify(g.layer):
-                    self.certify(g, twin[(g.layer, g.group)], kind, m, sd, k, sync=sync)
-                else:
-                    g.plan.pm_step(k, kind, m, sd, mode=self.mode, **sync)
-        for n, _ in enumerate(S.walk(it, seed, issue)):
-            li = S.schedule[n][0]
-            if li == snap_layer and (n + 1 == len(S.schedule) or S.schedule[n + 1][0] != li):
-                snap = self.get(self.E)
-        return snap
-
-    def twin_reference(self, labels, seed, upto, tag=False):
-        """The twin's uninterrupted sweep (PMSweep.init / iteration_by_group): the state after the initialisation (upto = None) or
-        at the end of layer upto[1] of iteration upto[0], iterations 0 .. upto[0] run in full."""
-        Sq = self.Sq
-        Sq.begin()
-        Sq.init(labels)
-        if tag:
-            self.tag(self.Eq)
-        if upto is None:
-            return self.get(self.Eq)
-        ref = None
-        for it in range(upto[0] + 1):
-            for n, _ in enumerate(Sq.iteration_by_group(it, seed)):
-                li = Sq.schedule[n][0]
-                if (it, li) == tuple(upto) and (n + 1 == len(Sq.schedule) or Sq.schedule[n + 1][0] != li):
-                    ref = self.get(self.Eq)
-        return ref
-
-
-def assert_same_state(a, b, what):
-    assert np.array_equal(bits(a[0]), bits(b[0])), f"{what}: currentCost differs at {int((bits(a[0]) != bits(b[0])).sum())} pixels"
-    assert np.array_equal(bits(a[1]), bits(b[1])), f"{what}: currentLabeling differs"
-
-
-def run_sweep(R, labels, iterations, seed, tag=True, what="scene"):
-    """The twin uninterrupted, then the sweep under test step by step with every step certified (the initialisation included);
-    the final states must be bit-identical."""
-    ref = R.twin_reference(labels, seed, (iterations - 1, len(R.S.unit_sizes) - 1), tag=tag)
-    R.E.pm_begin(R.mode)
-    R.init(labels)
-    if tag:
-        R.tag(R.E)
-    for it in range(iterations):
-        R.iteration(it, seed)
-    assert_same_state(R.get(R.E), ref, f"{what}: step by step against uninterrupted")
-    print(R.T.line(what))
-    return R.T
 
 
 # ---- designed scenes (small) -------------------------------------------------------------------------------------------------------------
@@ -467,8 +206,8 @@ def test_every_step_of_the_benchmark_workload(bench_rig, it, layer):
         state = R.get(R.E)
     else:
         for i in range(it):
-            R.iteration(i, BENCH_SEED, certify=lambda li: False)
-        state = R.iteration(it, BENCH_SEED, certify=lambda li: li == layer, snap_layer=layer)
+            R.iteration(i, BENCH_SEED, certify=lambda g: False)
+        state = R.iteration(it, BENCH_SEED, certify=lambda g: g.layer == layer, snap_layer=layer)[1]
     what = "benchmark workload, " + ("initialisation" if it is None else f"iteration {it}, layer {layer}")
     assert_same_state(state, ref, what)
     print(R.T.line(what) + f"; {time.perf_counter() - t0:.1f} s in all")

@@ -1,4 +1,4 @@
-"""The contract of the device RansacProposer as tests/ransac_oracle.py states it (DESIGN.md section 3f), checked on the CPU:
+"""The contract of the device RansacProposer as oracle/ransac_oracle.py states it (DESIGN.md section 3f), checked on the CPU:
 the solve against numpy's float64 least squares and OpenCV's own float cv::solve(DECOMP_SVD), computeSampleCount's edge cases, and
 the sampler's triples."""
 import math
@@ -6,7 +6,7 @@ import math
 import numpy as np
 import pytest
 
-import ransac_oracle as RO
+from oracle import ransac_oracle as RO
 from oracle import lexp_oracle as O
 
 

@@ -1,4 +1,4 @@
-"""tests/ransac_oracle.py against the reference's own RansacProposer (Proposer.h:155-312), compiled from its header into
+"""oracle/ransac_oracle.py against the reference's own RansacProposer (Proposer.h:155-312), compiled from its header into
 oracle/_ref/liblexp_ref_ransac.so (oracle/build_ref_ransac.py) over the shim's cv:: layer, whose cv::solve is the contract's double
 solve.  The samples' triples are injected into the reference's std::random_shuffle through the library's own rand(), so the
 reference runs RANSACPlane's control flow on the oracle's samples: the number of samples drawn, every inlier count (no_i, and no after
@@ -8,7 +8,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-import ransac_oracle as RO
+from oracle import ransac_oracle as RO
 import test_gpu_ransac as _gr
 from oracle import lexp_oracle as O
 

@@ -13,6 +13,7 @@
 #include "StereoEnergy.h"
 #endif
 #include <atomic>
+#include <cstring>
 #include <mutex>
 #include <stdexcept>
 #include <string>
@@ -22,6 +23,13 @@
 class CudaCostVolumeEnergy : public StereoEnergy {
 protected:
     lexp_ctx* ctx_ = nullptr;
+    int height_ = 0, width_ = 0;
+    std::vector<int> unitSizes_;                                     // addLayer / run
+    std::vector<std::vector<std::pair<int, int>>> layerProposers_;
+    uint64_t runSeed_ = 0;
+    float runPrecision_ = -1.0f, runThreshold_ = 0.5f;
+    lexp_run_callback runCallback_ = nullptr;
+    void* runUser_ = nullptr;
 
     static void check(int rc) {
         if (rc != LEXP_OK) throw std::runtime_error(std::string("lexp_cuda: ") + lexp_last_error());
@@ -55,7 +63,7 @@ protected:
         if (params.filterName != "GF" && params.filterName != "GFfloat")
             throw std::invalid_argument("the CUDA energies implement the guided-filter aggregation only");
         lexp_params p{};
-        p.height = imL.rows; p.width = imL.cols; p.ndisp = ndisp;
+        p.height = height_ = imL.rows; p.width = width_ = imL.cols; p.ndisp = ndisp;
         p.windR = params.windR; p.eps = params.filter_param1; p.th_col = params.th_col;
         p.min_disp = MIN_DISPARITY; p.max_disp = MAX_DISPARITY; p.device = device;
         p.energy_kind = energy_kind; p.alpha = params.alpha; p.th_grad = params.th_grad;
@@ -117,6 +125,43 @@ public:
     // PMStereoBase::postProcess(currentLabeling_[0], currentLabeling_[1], threshold) (PMStereoBase.h:146-256) on the device state of both
     // views (PatchMatchPhase for each), in place: the tail of a two-view run (INTEGRATION.md section 4c).  Needs lexp_set_smoothness (omega).
     void postProcess(float threshold = 1.5f) const { check(lexp_post_process(ctx_, threshold, nullptr)); }
+
+    // FastGCStereo::addLayer(unitRegionSize, proposers) and FastGCStereo::run(maxIteration, viewModes, pmInit, labeling, rawlabeling)
+    // (FastGCStereo.h:86-92,133-222) in one device call (lexp_run, INTEGRATION.md section 4d).  Proposers as (LEXP_PROP_*, K) pairs.
+    // An empty `labeling` starts from random labels; a given H x W CV_32FC4 labeling is the start of every view.  On return `labeling` /
+    // `rawlabeling` hold view 0 after / before the post-processing (H x W CV_32FC4).  setRunOptions: the run seed (the reference seeds
+    // cv::theRNG() from the clock) and the Evaluator's precision / threshold with a callback at its points (lexp_set_ground_truth first).
+    void addLayer(int unitRegionSize, const std::vector<std::pair<int, int>>& proposers) {
+        unitSizes_.push_back(unitRegionSize);
+        layerProposers_.push_back(proposers);
+    }
+    void setRunOptions(uint64_t seed, float precision = -1.0f, float threshold = 0.5f, lexp_run_callback callback = nullptr, void* user = nullptr) {
+        runSeed_ = seed; runPrecision_ = precision; runThreshold_ = threshold; runCallback_ = callback; runUser_ = user;
+    }
+#ifdef CV_32FC4   // OpenCV's Mat::create / CV_32FC4 (a cv:: stand-in without them leaves run out)
+    void run(int maxIteration, const std::vector<int>& viewModes, int pmInit, cv::Mat& labeling, cv::Mat& rawlabeling) const {
+        const bool dual = viewModes.size() == 2 && viewModes[0] == 0 && viewModes[1] == 1;
+        if (!dual && !(viewModes.size() == 1 && viewModes[0] == 0)) throw std::invalid_argument("run: viewModes must be {0} or {0, 1}");
+        std::vector<int> np, kind, K;
+        for (const auto& pl : layerProposers_) {
+            np.push_back((int)pl.size());
+            for (const auto& p : pl) { kind.push_back(p.first); K.push_back(p.second); }
+        }
+        const bool given = labeling.data != nullptr;
+        if (given && (labeling.rows != height_ || labeling.cols != width_ || labeling.step != (size_t)width_ * sizeof(lexp_plane)))
+            throw std::invalid_argument("run: the given labeling must be a continuous H x W CV_32FC4 mat");
+        std::vector<lexp_plane> lab((size_t)height_ * width_), raw((size_t)height_ * width_);
+        lexp_run_options o{dual ? 2 : 1, pmInit, maxIteration, (int)unitSizes_.size(), unitSizes_.data(), np.data(), kind.data(), K.data(),
+                           given ? reinterpret_cast<const lexp_plane*>(labeling.data) : nullptr, runSeed_, runPrecision_, runThreshold_};
+        check(lexp_run(ctx_, &o, lab.data(), raw.data(), runCallback_, runUser_));
+        labeling.create(height_, width_, CV_32FC4);
+        rawlabeling.create(height_, width_, CV_32FC4);
+        for (int y = 0; y < height_; y++) {
+            std::memcpy(labeling.data + labeling.step * (size_t)y, &lab[(size_t)y * width_], (size_t)width_ * sizeof(lexp_plane));
+            std::memcpy(rawlabeling.data + rawlabeling.step * (size_t)y, &raw[(size_t)y * width_], (size_t)width_ * sizeof(lexp_plane));
+        }
+    }
+#endif
 
     lexp_ctx* context() const { return ctx_; }
     // error state of the per-cell virtuals (they never throw, see guard()): check after the OpenMP region

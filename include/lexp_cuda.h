@@ -347,6 +347,66 @@ LEXP_API int lexp_plan_gc_step(lexp_ctx* ctx, lexp_plan* plan, int mode, int kin
  * (lexp_pm_sweep_create with world == 1): lexp_plan_gc_step for every proposal step of every group.  Asynchronous. */
 LEXP_API int lexp_pm_sweep_gc_iteration(lexp_pm_sweep* sweep, int iteration, uint64_t seed, int* n_steps);
 
+/* ---- A whole run: FastGCStereo::run (FastGCStereo.h:133-222) with its random start and its Evaluator, on one GPU (DESIGN.md 3h).
+ *
+ * lexp_pm_sweep_init_random: initCurrentFast with an empty labeling (FastGCStereo.h:100-114).  A kernel draws one label per unit region
+ * of layer 0, one thread per unit: selectRandomPixelInRect + StereoEnergy::createRandomLabel (StereoEnergy.h:120-129, MAX_VDISPARITY = 0)
+ * from the cv::RNG stream pm_rng_state(seed, unit index) -- the stream a proposer of that cell would draw from with launch seed `seed`.
+ * The init step then reads the labels like the list of lexp_pm_sweep_init, and it behaves as that call does (lexp_pm_begin first;
+ * asynchronous for the cost-volume energy, returns after its launches for the image-based energy).  One GPU (world = 1). */
+LEXP_API int lexp_pm_sweep_init_random(lexp_pm_sweep* sweep, uint64_t seed);
+
+/* Evaluator (Evaluator.h): the left view's ground truth, float[H][W] disparities (0 or +inf: no ground truth), and its non-occlusion
+ * mask, uint8[H][W], of which the pixels equal to 255 count as non-occluded (main.cpp:262-265; NULL: every pixel).  Host arrays, copied
+ * to the device once; blocking. */
+LEXP_API int lexp_set_ground_truth(lexp_ctx* ctx, const float* gt_host, const uint8_t* nonocc_host);
+typedef struct lexp_eval_result {
+    double energy, data, smooth;       /* data + smooth; sum of currentCost_; computeSmoothnessCost (lexp_energy) */
+    int64_t valid_pixels;              /* GT > 0 & GT != inf                                                     */
+    int64_t nonocc_pixels;             /* the mask's pixels                                                       */
+    int64_t all_correct;               /* |disp - GT| <= threshold among the valid pixels                         */
+    int64_t nonocc_correct;            /* ... among the non-occluded pixels                                       */
+    double all, nonocc;                /* error rates in percent: 100 (1 - correct / pixels), as Evaluator.h:160-163 */
+} lexp_eval_result;
+/* Evaluator::evaluate(currentLabeling_m_[mode], currentCost_[mode], ...) (Evaluator.h:113-187) on the device state of view `mode`:
+ * disp = computeDisparities; with precision > 0 the Evaluator's quantize (convertTo CV_32S: disp * (float)(1.0 / precision) in float,
+ * cvRound = round half to even; then back with scale precision in double, rounded to float); a pixel is correct where |disp - GT| <= threshold.
+ * Like the reference, every view is compared against the left view's ground truth.  One pixel-parallel launch with integer counts per
+ * block, added in block order: the same result on every call.  Blocking.  LEXP_ERR_STATE without lexp_set_ground_truth. */
+LEXP_API int lexp_evaluate(lexp_ctx* ctx, int mode, float precision, float threshold, lexp_eval_result* out);
+
+typedef struct lexp_run_options {
+    int n_views;            /* 1: viewModes {0}; 2: {0, 1} (-doDual) with the post-processing of both views at the end          */
+    int pm_iterations;      /* pmInit: PatchMatch iterations (FastGCStereo.h:143-157)                                           */
+    int iterations;         /* maxIteration: graph-cut iterations (FastGCStereo.h:171-184)                                       */
+    int n_layers;           /* layers and proposer lists as lexp_pm_sweep_create takes them                                      */
+    const int* unit_sizes;
+    const int* n_proposers;
+    const int* proposer_kind;
+    const int* proposer_K;
+    const lexp_plane* init_labeling;  /* NULL: random start; else Plane[H][W] every view starts from (FastGCStereo.h:116-130, 3g)  */
+    uint64_t seed;          /* run seed: every phase's stream derives from it (lexp_run_seed)                                    */
+    float precision;        /* for the callback's lexp_evaluate                                                                  */
+    float threshold;
+} lexp_run_options;
+/* index: the Evaluator's index (0 after init, it + 1 after pm iteration it, it + 1 + pm_iterations after graph-cut iteration it,
+ * iterations + 1 + pm_iterations after the post-processing, for view 0 then view 1).  seconds: the run's timer at that point -- it starts
+ * after the initialisation and does not run during evaluations (FastGCStereo.h:141, Evaluator.h:115-116). */
+typedef void (*lexp_run_callback)(void* user, int index, int mode, const lexp_eval_result* result, double seconds);
+/* The seed of one phase of a run: phase 0 = initialisation (the seed of lexp_pm_sweep_init_random; `iteration` ignored), 1 = pm
+ * iteration, 2 = graph-cut iteration (the seed of lexp_pm_sweep_iteration / lexp_pm_sweep_gc_iteration).  A splitmix64 hash of
+ * (run_seed, mode, phase, iteration): distinct streams for every view, phase and iteration. */
+LEXP_API uint64_t lexp_run_seed(uint64_t run_seed, int mode, int phase, int iteration);
+/* FastGCStereo::run(iterations, viewModes, pm_iterations, labeling, rawlabeling) on the device: for every view lexp_pm_begin and the
+ * initialisation (lexp_pm_sweep_init_random, or lexp_pm_begin with init_labeling + lexp_pm_init_from_labeling), then the pm iterations
+ * (lexp_pm_sweep_iteration) and the graph-cut iterations (lexp_pm_sweep_gc_iteration) view after view, and with two views the raw labeling
+ * of view 0 followed by lexp_post_process(1.5).  Seeds from lexp_run_seed.  The smoothness parameters are the context's
+ * (lexp_set_smoothness; two views need it for the post-processing).  labeling_out / raw_out (nullable): Plane[H][W] of view 0 after /
+ * before the post-processing (the same with one view).  callback (nullable; needs lexp_set_ground_truth) is invoked at the Evaluator's
+ * points with lexp_evaluate(ctx, mode, precision, threshold).  Blocking.  The device state of the views stays for further calls. */
+LEXP_API int lexp_run(lexp_ctx* ctx, const lexp_run_options* options, lexp_plane* labeling_out, lexp_plane* raw_out,
+                      lexp_run_callback callback, void* user);
+
 /* LayerManager::addLayer (LayerManager.h:44-185): cell geometry of one layer.
  * Call with rect pointers == NULL to query counts.  group_of[r] = (i%4)*4 + (j%4) (LayerManager.h:168-173). */
 LEXP_API int lexp_layer_geometry(int width, int height, int windR, int unit_size, int* height_blocks,

@@ -29,6 +29,21 @@ class Params(C.Structure):
                 ("energy_kind", C.c_int), ("alpha", C.c_float), ("th_grad", C.c_float), ("reserved", C.c_int * 4)]
 
 
+class EvalResult(C.Structure):  # lexp_eval_result
+    _fields_ = [("energy", C.c_double), ("data", C.c_double), ("smooth", C.c_double), ("valid_pixels", C.c_int64),
+                ("nonocc_pixels", C.c_int64), ("all_correct", C.c_int64), ("nonocc_correct", C.c_int64), ("all", C.c_double),
+                ("nonocc", C.c_double)]
+
+
+class RunOptions(C.Structure):  # lexp_run_options
+    _fields_ = [("n_views", C.c_int), ("pm_iterations", C.c_int), ("iterations", C.c_int), ("n_layers", C.c_int),
+                ("unit_sizes", C.c_void_p), ("n_proposers", C.c_void_p), ("proposer_kind", C.c_void_p), ("proposer_K", C.c_void_p),
+                ("init_labeling", C.c_void_p), ("seed", C.c_uint64), ("precision", C.c_float), ("threshold", C.c_float)]
+
+
+# lexp_run_callback(user, index, mode, result, seconds)
+RUN_CALLBACK = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.POINTER(EvalResult), C.c_double)
+
 # every symbol include/lexp_cuda.h declares: (restype, argtypes)
 _P = C.c_void_p
 SYMBOLS = {
@@ -91,6 +106,11 @@ SYMBOLS = {
     "lexp_post_process": (C.c_int, [_P, C.c_float, _P]),
     "lexp_energy": (C.c_int, [_P, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "lexp_plan_gc_step": (C.c_int, [_P, _P, C.c_int, C.c_int, C.c_int, C.c_uint64, _P, C.c_int, _P, _P]),
+    "lexp_pm_sweep_init_random": (C.c_int, [_P, C.c_uint64]),
+    "lexp_set_ground_truth": (C.c_int, [_P, _P, _P]),
+    "lexp_evaluate": (C.c_int, [_P, C.c_int, C.c_float, C.c_float, C.POINTER(EvalResult)]),
+    "lexp_run_seed": (C.c_uint64, [C.c_uint64, C.c_int, C.c_int, C.c_int]),
+    "lexp_run": (C.c_int, [_P, C.POINTER(RunOptions), _P, _P, RUN_CALLBACK, _P]),
     "lexp_layer_geometry": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), _P, _P, _P, _P]),
 }
 

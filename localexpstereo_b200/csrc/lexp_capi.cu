@@ -7,6 +7,7 @@
 #include "lexp_post.cuh"
 #include "lexp_ransac.cuh"
 #include "lexp_label_cost.cuh"
+#include "lexp_run.cuh"
 
 #include <algorithm>
 #include <cstdio>
@@ -141,6 +142,8 @@ struct lexp_ctx {
     int* h_gc_flags = nullptr;                     // pinned: the two decision flags of the phase path
     char* d_post = nullptr;                        // lexp_post_process scratch: filled labelings, fail maps, row counts / offsets, list, weights
     float* d_ransac_disp = nullptr;                // LEXP_PROP_RANSAC: float[H][W], the disparities of the snapshot of every cell's unitRegion
+    float* d_gt = nullptr;                         // lexp_set_ground_truth: the left view's GT disparities float[H][W]
+    unsigned char* d_nonocc = nullptr;             //                        and its non-occlusion mask (1: nonocc == 255)
     int64_t launches = 0;
     int64_t overlapped_launches = 0;   // fused launches that carried the programmatic-serialization attribute
     int64_t lean_launches = 0;         // fused launches of the lean build (kLeanCtas)
@@ -715,6 +718,8 @@ int lexp_destroy(lexp_ctx* c) {
     cudaFree(c->d_gc_scratch);
     cudaFree(c->d_post);
     cudaFree(c->d_ransac_disp);
+    cudaFree(c->d_gt);
+    cudaFree(c->d_nonocc);
     if (c->h_gc_flags) cudaFreeHost(c->h_gc_flags);
     cudaFree(c->d_sync_arena);
     if (c->own_stream) cudaStreamDestroy(c->stream);
@@ -1873,11 +1878,12 @@ uint64_t pm_launch_seed(uint64_t base, int mode, int iteration, int layer, int g
     z = (z ^ (z >> 33)) * 0xFF51AFD7ED558CCDull;
     return z ^ (z >> 29);
 }
-int sweep_step(lexp_pm_sweep* s, lexp_plan* plan, int step_index, int kind, int m, uint64_t seed, const lexp_plane* planes, int flags, bool first, bool last) {
+int sweep_step(lexp_pm_sweep* s, lexp_plan* plan, int step_index, int kind, int m, uint64_t seed, const lexp_plane* planes, int flags, bool first, bool last,
+               int planes_on_device = 0) {
     int we[kMaxPeers];
     unsigned mask = 0;
     for (int r = 0; r < kMaxPeers; r++) { we[r] = s->has[r] ? s->last_rel[r] : 0; if (first && s->has[r]) mask |= 1u << r; }
-    return lexp_plan_pm_step_ex(s->ctx, plan, s->mode, step_index, kind, m, seed, planes, 0, nullptr, flags, last ? s->rel + 1 : 0, we, mask);
+    return lexp_plan_pm_step_ex(s->ctx, plan, s->mode, step_index, kind, m, seed, planes, planes_on_device, nullptr, flags, last ? s->rel + 1 : 0, we, mask);
 }
 void sweep_group_done(lexp_pm_sweep* s, const std::vector<int>& owners) {
     s->rel++;
@@ -2048,6 +2054,139 @@ int lexp_pm_sweep_gc_iteration(lexp_pm_sweep* s, int iteration, uint64_t seed, i
     }
     if (n_steps) *n_steps = steps_done;
     return LEXP_OK;
+}
+
+// ---- a whole run (FastGCStereo::run, FastGCStereo.h:133-222): random start, Evaluator, and the run itself ---------------------------
+
+// initCurrentFast with an empty labeling: the random-start kernel (lexp_run.cuh) writes one label per layer-0 unit into the init plan's
+// plane buffer, which the init step reads like a list.  The kernel is an ordinary launch, so the fused launch after it does not overlap it.
+int lexp_pm_sweep_init_random(lexp_pm_sweep* s, uint64_t seed) {
+    if (!s) return fail(LEXP_ERR_INVALID, "bad argument");
+    if (s->world != 1 || !s->init_plan) return fail(LEXP_ERR_INVALID, "the random start runs on one GPU (world = 1)");
+    lexp_ctx* c = s->ctx;
+    lexp_plan* pl = s->init_plan;
+    { int rc = require_pm_state(c, s->mode); if (rc) return rc; }
+    int rc = lexp_pm_reset_sync(c);
+    if (rc) return rc;
+    {
+        LEXP_ENTER(c);
+        LEXP_CUDA(launch_aux(c, lexp_random_start_kernel, (pl->ncalls + 127) / 128, 128, pl->d_calls, pl->ncalls, pl->d_planes, (unsigned long long)seed,
+                             c->p.min_disp, c->p.max_disp));
+    }
+    const lexp_plane* dp = reinterpret_cast<const lexp_plane*>(pl->d_planes);
+    if (c->p.energy_kind != 0) {   // the image-based energy: unary launch + assignment, as lexp_pm_sweep_init
+        rc = lexp_plan_init_step(c, pl, s->mode, dp, 1);
+        return rc ? rc : lexp_sync(c);
+    }
+    rc = sweep_step(s, pl, 0, LEXP_PROP_LIST, 0, 0, dp, LEXP_PM_INIT, true, true, 1);
+    if (rc) return rc;
+    sweep_group_done(s, s->init_owners);
+    return sweep_advance(s);
+}
+
+int lexp_set_ground_truth(lexp_ctx* c, const float* gt, const uint8_t* nonocc) {
+    if (!c || !gt) return fail(LEXP_ERR_INVALID, "bad argument");
+    LEXP_ENTER(c);
+    const size_t HW = (size_t)c->p.height * c->p.width;
+    std::vector<unsigned char> mask(HW, 1);
+    if (nonocc)
+        for (size_t i = 0; i < HW; i++) mask[i] = nonocc[i] == 255;   // nonocc = nonocc == 255 (main.cpp:262-263)
+    if (!c->d_gt) LEXP_CUDA(cudaMalloc(&c->d_gt, HW * sizeof(float)));
+    if (!c->d_nonocc) LEXP_CUDA(cudaMalloc(&c->d_nonocc, HW));
+    LEXP_CUDA(h2d(c, c->d_gt, gt, HW * sizeof(float)));
+    LEXP_CUDA(h2d(c, c->d_nonocc, mask.data(), HW));
+    LEXP_CUDA(cudaStreamSynchronize(c->stream));
+    return LEXP_OK;
+}
+
+int lexp_evaluate(lexp_ctx* c, int mode, float precision, float threshold, lexp_eval_result* out) {
+    if (!c || !out || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
+    if (!c->d_gt) return fail(LEXP_ERR_STATE, "lexp_set_ground_truth has not been called");
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    double data = 0.0, smooth = 0.0;
+    { int rc = lexp_energy(c, mode, &data, &smooth); if (rc) return rc; }   // the Evaluator's dc2 / sc2 (Evaluator.h:119-121)
+    LEXP_ENTER(c);
+    const int H = c->p.height, W = c->p.width;
+    const int nblocks = (int)(((size_t)H * W + kEvalThreads - 1) / kEvalThreads);
+    long long n[4] = {0, 0, 0, 0};
+    const int rc = read_back(c, "lexp_evaluate", (4 * (size_t)nblocks + 4) * sizeof(long long), 4 * (size_t)nblocks * sizeof(long long), n, sizeof(n), [&](char* d) {
+        long long* d_part = reinterpret_cast<long long*>(d);
+        cudaError_t e = launch_aux(c, lexp_eval_kernel, nblocks, kEvalThreads, c->d_cur_label[mode], c->d_gt, c->d_nonocc, d_part, H, W, precision, threshold);
+        return e == cudaSuccess ? launch_aux(c, lexp_eval_finish, 1, 4, d_part, nblocks, d_part + 4 * (size_t)nblocks) : e;
+    });
+    if (rc) return rc;
+    out->data = data; out->smooth = smooth; out->energy = smooth + data;   // eng2 = sc2 + dc2
+    out->valid_pixels = n[0]; out->nonocc_pixels = n[1]; out->all_correct = n[2]; out->nonocc_correct = n[3];
+    out->all = (1.0 - (double)n[2] / (double)n[0]) * 100.0;              // Evaluator.h:160-163
+    out->nonocc = (1.0 - (double)n[3] / (double)n[1]) * 100.0;
+    return LEXP_OK;
+}
+
+uint64_t lexp_run_seed(uint64_t run_seed, int mode, int phase, int iteration) {   // = localexpstereo_b200.sweep.run_seed
+    uint64_t z = run_seed * 0x9E3779B97F4A7C15ull + (uint64_t)(mode + 1) * 0xC2B2AE3D27D4EB4Full + (uint64_t)(phase + 1) * 0x165667B19E3779F9ull +
+                 (uint64_t)(phase == 0 ? 0 : iteration + 1) * 0x27D4EB2F165667C5ull;
+    z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+    z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+    return z ^ (z >> 31);
+}
+
+int lexp_run(lexp_ctx* c, const lexp_run_options* o, lexp_plane* labeling_out, lexp_plane* raw_out, lexp_run_callback callback, void* user) {
+    if (!c || !o || (o->n_views != 1 && o->n_views != 2) || o->pm_iterations < 0 || o->iterations < 0) return fail(LEXP_ERR_INVALID, "bad argument");
+    if (callback && !c->d_gt) return fail(LEXP_ERR_STATE, "the callback evaluates the run: lexp_set_ground_truth first");
+    if (o->n_views == 2 && !c->sm_set) return fail(LEXP_ERR_STATE, "lexp_set_smoothness has not been called: the post-processing needs omega");
+    const int nv = o->n_views;
+    std::vector<lexp_pm_sweep*> sw(nv, nullptr);
+    auto done = [&](int rc) -> int { for (lexp_pm_sweep* s : sw) lexp_pm_sweep_destroy(s); return rc; };
+    for (int m = 0; m < nv; m++) {
+        int rc = lexp_pm_sweep_create(c, m, o->n_layers, o->unit_sizes, o->n_proposers, o->proposer_kind, o->proposer_K, 0, 1, &sw[m]);
+        if (rc) return done(rc);
+    }
+    // the Evaluator's timer (TimeStamper): runs from the end of the initialisation, stopped while evaluating
+    using clk = std::chrono::steady_clock;
+    double elapsed = 0.0;
+    clk::time_point t0;
+    bool ticking = false;
+    auto evaluate = [&](int index, int mode) -> int {
+        int rc = lexp_sync(c);
+        if (ticking) elapsed += std::chrono::duration<double>(clk::now() - t0).count();
+        if (rc || !callback) { t0 = clk::now(); return rc; }
+        lexp_eval_result r{};
+        rc = lexp_evaluate(c, mode, o->precision, o->threshold, &r);
+        if (rc) return rc;
+        callback(user, index, mode, &r, elapsed);
+        t0 = clk::now();
+        return LEXP_OK;
+    };
+    for (int m = 0; m < nv; m++) {   // currentCost_ = INFINITY; initCurrentFast (:135-139)
+        int rc = lexp_pm_begin(c, m, nullptr, o->init_labeling);
+        if (!rc) rc = o->init_labeling ? lexp_pm_init_from_labeling(c, m) : lexp_pm_sweep_init_random(sw[m], lexp_run_seed(o->seed, m, 0, 0));
+        if (!rc) rc = evaluate(0, m);
+        if (rc) return done(rc);
+    }
+    t0 = clk::now();
+    ticking = true;
+    for (int it = 0; it < o->pm_iterations; it++)   // :143-157
+        for (int m = 0; m < nv; m++) {
+            int rc = lexp_pm_sweep_iteration(sw[m], it, lexp_run_seed(o->seed, m, 1, it), nullptr);
+            if (!rc) rc = evaluate(it + 1, m);
+            if (rc) return done(rc);
+        }
+    for (int it = 0; it < o->iterations; it++)      // :171-184
+        for (int m = 0; m < nv; m++) {
+            int rc = lexp_pm_sweep_gc_iteration(sw[m], it, lexp_run_seed(o->seed, m, 2, it), nullptr);
+            if (!rc) rc = evaluate(it + 1 + o->pm_iterations, m);
+            if (rc) return done(rc);
+        }
+    if (nv == 2) {   // rawlabeling = currentLabeling_[0].clone(); postProcess(.., 1.5) (:199-205)
+        int rc = raw_out ? lexp_pm_get(c, 0, nullptr, raw_out) : LEXP_OK;
+        if (!rc) rc = lexp_post_process(c, 1.5f, nullptr);
+        for (int m = 0; m < 2 && !rc; m++) rc = evaluate(o->iterations + 1 + o->pm_iterations, m);
+        if (!rc && labeling_out) rc = lexp_pm_get(c, 0, nullptr, labeling_out);
+        return done(rc);
+    }
+    int rc = labeling_out ? lexp_pm_get(c, 0, nullptr, labeling_out) : LEXP_OK;
+    if (!rc && raw_out) rc = lexp_pm_get(c, 0, nullptr, raw_out);
+    return done(rc);
 }
 
 // LayerManager::addLayer, LayerManager.h:88-185 (the #else branch that merges small edge cells).

@@ -384,6 +384,65 @@ class CostVolumeEnergy:
         check(lib().lexp_energy(self._h, mode, C.byref(d), C.byref(s)))
         return d.value, s.value
 
+    # --- a whole run: FastGCStereo::run with the Evaluator (lexp_set_ground_truth / lexp_evaluate / lexp_run) ---------------------
+    def set_ground_truth(self, gt, nonocc=None):
+        """The left view's ground truth for `evaluate` / `run`: float32 [H][W] disparities (0 or inf: none) and the uint8 [H][W]
+        non-occlusion mask, of which the pixels equal to 255 count (None: every pixel)."""
+        g = np.ascontiguousarray(gt, dtype=np.float32)
+        m = None if nonocc is None else np.ascontiguousarray(nonocc, dtype=np.uint8)
+        assert g.shape == (self.height, self.width) and (m is None or m.shape == g.shape)
+        check(lib().lexp_set_ground_truth(self._h, g.ctypes.data, None if m is None else m.ctypes.data))
+
+    @staticmethod
+    def _eval_dict(r) -> dict:
+        return {k: getattr(r, k) for k, _ in _capi.EvalResult._fields_}
+
+    def evaluate(self, mode=0, precision=-1.0, threshold=0.5) -> dict:
+        """Evaluator::evaluate (Evaluator.h:113-187) on the device state of view `mode` against the left ground truth: energy, data,
+        smooth, the pixel counts (valid_pixels, nonocc_pixels, all_correct, nonocc_correct) and the error rates all / nonocc in percent.
+        precision > 0 quantises the disparities to multiples of it first."""
+        r = _capi.EvalResult()
+        check(lib().lexp_evaluate(self._h, int(mode), float(precision), float(threshold), C.byref(r)))
+        return self._eval_dict(r)
+
+    def run(self, maxIteration, viewModes=(0, 1), pmInit=0, labeling=None, unit_sizes=None, proposers=None, seed=0, precision=-1.0,
+            threshold=0.5, callback=None):
+        """FastGCStereo::run(maxIteration, viewModes, pmInit, labeling, rawlabeling) on the device (lexp_run): random start (or the
+        given Plane [H][W] labeling), pmInit PatchMatch iterations, maxIteration graph-cut iterations and, with viewModes (0, 1), the
+        post-processing.  unit_sizes / proposers: the layers and their [(kind, K)] lists (default: sweep.v3_layer_units and
+        sweep.V3_PROPOSERS_REFERENCE).  callback(index, mode, result_dict, seconds) at the Evaluator's points (set_ground_truth first).
+        Returns (labeling, rawlabeling) of view 0, float32 [H][W][4] each."""
+        from .sweep import V3_PROPOSERS_REFERENCE, v3_layer_units
+        views = tuple(viewModes)
+        if views not in ((0,), (0, 1)):
+            raise LexpError("viewModes must be (0,) or (0, 1)")
+        units = np.ascontiguousarray(unit_sizes if unit_sizes is not None else v3_layer_units(self.width), dtype=np.int32)
+        props = proposers if proposers is not None else V3_PROPOSERS_REFERENCE
+        n_prop = np.ascontiguousarray([len(p) for p in props], dtype=np.int32)
+        kinds = np.ascontiguousarray([k for p in props for k, _ in p], dtype=np.int32)
+        Ks = np.ascontiguousarray([K for p in props for _, K in p], dtype=np.int32)
+        init = None
+        if labeling is not None:
+            init = np.ascontiguousarray(labeling, dtype=np.float32)
+            assert init.shape == (self.height, self.width, 4)
+        o = _capi.RunOptions(len(views), int(pmInit), int(maxIteration), len(units), units.ctypes.data, n_prop.ctypes.data, kinds.ctypes.data,
+                             Ks.ctypes.data, None if init is None else init.ctypes.data, int(seed) & 0xFFFFFFFFFFFFFFFF, float(precision),
+                             float(threshold))
+        lab = np.empty((self.height, self.width, 4), np.float32)
+        raw = np.empty((self.height, self.width, 4), np.float32)
+        errors = []
+
+        def tramp(_user, index, mode, res, seconds):
+            try:
+                callback(int(index), int(mode), self._eval_dict(res.contents), float(seconds))
+            except BaseException as e:   # an exception cannot cross the C frames: re-raised after the run
+                errors.append(e)
+        cb = _capi.RUN_CALLBACK(tramp) if callback is not None else _capi.RUN_CALLBACK()
+        check(lib().lexp_run(self._h, C.byref(o), lab.ctypes.data, raw.ctypes.data, cb, None))
+        if errors:
+            raise errors[0]
+        return lab, raw
+
     # --- PatchMatch phase state: currentCost_[mode] / currentLabeling_[mode] resident on the device ------------------------
     def pm_begin(self, mode=0, cost=None, labeling=None):
         """FastGCStereo::run, :137: currentCost_ = INFINITY (or `cost`), currentLabeling_ = `labeling` (or zeros)."""

@@ -138,6 +138,20 @@ def pm_seed(base, mode, iteration, layer, group, step):
     return z ^ (z >> 29)
 
 
+RUN_INIT, RUN_PM, RUN_GC = 0, 1, 2   # phases of a run (lexp_run_seed)
+
+
+def run_seed(base, mode, phase, iteration=0):
+    """Seed of one phase of a whole run (= lexp_run_seed): RUN_INIT (the random start's seed; iteration ignored), RUN_PM / RUN_GC (the
+    base seed of pm / graph-cut iteration `iteration`, which pm_seed then hashes per launch)."""
+    M = 0xFFFFFFFFFFFFFFFF
+    z = (int(base) * 0x9E3779B97F4A7C15 + (mode + 1) * 0xC2B2AE3D27D4EB4F + (phase + 1) * 0x165667B19E3779F9
+         + (0 if phase == RUN_INIT else iteration + 1) * 0x27D4EB2F165667C5) & M
+    z = ((z ^ (z >> 30)) * 0xBF58476D1CE4E5B9) & M
+    z = ((z ^ (z >> 27)) * 0x94D049BB133111EB) & M
+    return z ^ (z >> 31)
+
+
 def expand_proposers(proposers, outer_iter, max_disp, min_disp=0.0):
     """[(kind, K)] -> the proposal steps [(kind, m)] of one cell visit, as the `while (prop->isContinued())` loops of
     FastGCStereo.h:41-46 produce them; RandomProposer stops early when its disparity perturbation width falls below 0.1
@@ -367,6 +381,12 @@ class NativePMSweep:
         lb = np.ascontiguousarray(labels, dtype=np.float32)
         assert lb.shape == (self.num_init_labels, 4)
         check(lib().lexp_pm_sweep_init(self._h, lb.ctypes.data))
+
+    def random_start(self, seed):
+        """initCurrentFast with an empty labeling (lexp_pm_sweep_init_random): a random plane through a random pixel of every layer-0
+        unit, drawn on the device from the stream pm_rng_state(seed, unit index); begin() first."""
+        from ._capi import check, lib
+        check(lib().lexp_pm_sweep_init_random(self._h, int(seed) & 0xFFFFFFFFFFFFFFFF))
 
     def iteration(self, iteration, seed):
         import ctypes as C

@@ -60,9 +60,8 @@ protected:
     CudaCostVolumeEnergy(const cv::Mat imL, const cv::Mat imR, Parameters params, float MAX_DISPARITY, float MIN_DISPARITY, float MAX_VDISPARITY,
                          int device, int energy_kind, int ndisp)
         : StereoEnergy(imL, imR, params, MAX_DISPARITY, MIN_DISPARITY, MAX_VDISPARITY) {
-        if (params.filterName != "GF" && params.filterName != "GFfloat")
-            throw std::invalid_argument("the CUDA energies implement the guided-filter aggregation only");
         lexp_params p{};
+        p.filter = filterKind(params.filterName, energy_kind);
         p.height = height_ = imL.rows; p.width = width_ = imL.cols; p.ndisp = ndisp;
         p.windR = params.windR; p.eps = params.filter_param1; p.th_col = params.th_col;
         p.min_disp = MIN_DISPARITY; p.max_disp = MAX_DISPARITY; p.device = device;
@@ -73,6 +72,19 @@ protected:
     }
 
 public:
+    // Parameters::filterName as the reference's energies select their filter (CostVolumeEnergy.h:23-42, StereoEnergy.h:666-686).  The
+    // names for which the reference leaves its filter a null pointer ("BF" with the cost-volume energy, "BL" with the image-based one,
+    // anything unknown) crash it in ComputeUnaryPotential: rejected here.
+    static int filterKind(const std::string& name, int energy_kind) {
+        if (name == "GF" || name == "GFfloat") return LEXP_FILTER_GF;
+        if (name.empty()) return LEXP_FILTER_NONE;
+        if (name == (energy_kind == 0 ? "BL" : "BF")) return LEXP_FILTER_BILATERAL;
+        throw std::invalid_argument(std::string("filterName \"") + name + "\": the reference's " +
+                                    (energy_kind == 0 ? "CostVolumeEnergy" : "NaiveStereoEnergy") +
+                                    " leaves its filter a null pointer for this name (valid: \"GF\", \"GFfloat\", \"" +
+                                    (energy_kind == 0 ? "BL" : "BF") + "\", \"\")");
+    }
+
     // same argument list as CostVolumeEnergy::CostVolumeEnergy (CostVolumeEnergy.h:16)
     CudaCostVolumeEnergy(const cv::Mat imL, const cv::Mat imR, const cv::Mat volL, const cv::Mat volR, Parameters params,
                          float MAX_DISPARITY, float MIN_DISPARITY = 0, float MAX_VDISPARITY = 0, int device = 0)

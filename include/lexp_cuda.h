@@ -56,8 +56,27 @@ typedef struct lexp_params {
     int energy_kind;    /* 0: CostVolumeEnergy (CostVolumeEnergy.h:6-184); 1: NaiveStereoEnergy (StereoEnergy.h:629-764), no volume */
     float alpha;        /* Parameters::alpha   (NaiveStereoEnergy only, StereoEnergy.h:659-664)   */
     float th_grad;      /* Parameters::th_grad (NaiveStereoEnergy only)                            */
-    int reserved[4];
+    int filter;         /* aggregation filter, LEXP_FILTER_* (0 = the guided filter)                */
+    int reserved[3];
 } lexp_params;
+
+/* Aggregation filter of the unary term (Parameters::filterName, StereoEnergy.h:24).  The reference's names per energy:
+ *   CostVolumeEnergy  (CostVolumeEnergy.h:23-42):  "GF", "GFfloat" -> LEXP_FILTER_GF;  "BL" -> LEXP_FILTER_BILATERAL;  "" -> LEXP_FILTER_NONE
+ *   NaiveStereoEnergy (StereoEnergy.h:666-686):    "GF", "GFfloat" -> LEXP_FILTER_GF;  "BF" -> LEXP_FILTER_BILATERAL;  "" -> LEXP_FILTER_NONE
+ * Every other name ("BF" with CostVolumeEnergy, "BL" with NaiveStereoEnergy, anything unknown) leaves the reference's filter a null
+ * pointer that ComputeUnaryPotential dereferences: the adapters reject those names.
+ *   LEXP_FILTER_GF         guided filter, box radius windR / 2, eps = Parameters::filter_param1 (GuidedFilter.h:58-243).
+ *   LEXP_FILTER_BILATERAL  BilateralFilter (GuidedFilter.h:329-373): q(x) = sum over y in (x +- windR) & filterRect of
+ *                          p(y) exp(-|I(y) - I(x)|_1 / sig2) with the 8-bit BGR guide unscaled, not normalised; `eps` carries
+ *                          sig2 = Parameters::filter_param1 (> 0 and finite, else lexp_create returns LEXP_ERR_INVALID).
+ *   LEXP_FILTER_NONE       no filter: the raw cost itself (CostVolumeEnergy.h:169-171, StereoEnergy.h:752-753); `eps` unused.
+ * Every entry point works with every filter, except the multi-GPU cell shard (lexp_pm_ipc_connect / lexp_pm_connect_local return
+ * LEXP_ERR_INVALID on a context whose filter is not LEXP_FILTER_GF).  lexp_get_stats returns the guided-filter statistics of the guide
+ * whatever the filter.  lexp_plan_pm_step[_ex] on a context without the guided filter runs as proposals, unary costs and an update launch;
+ * lexp_plan_set_units prepares what those need, so the steps stay graph-capturable.  DESIGN.md section 3i. */
+#define LEXP_FILTER_GF 0
+#define LEXP_FILTER_BILATERAL 1
+#define LEXP_FILTER_NONE 2
 
 typedef struct lexp_ctx lexp_ctx;   /* replaces a CostVolumeEnergy instance (CostVolumeEnergy.h:6-184) */
 typedef struct lexp_plan lexp_plan; /* device-side work list for a fixed set of (filterRect, targetRect) */

@@ -26,7 +26,11 @@ class PlaneC(C.Structure):  # Plane.h:4-8
 class Params(C.Structure):
     _fields_ = [("height", C.c_int), ("width", C.c_int), ("ndisp", C.c_int), ("windR", C.c_int), ("eps", C.c_float),
                 ("th_col", C.c_float), ("min_disp", C.c_float), ("max_disp", C.c_float), ("device", C.c_int),
-                ("energy_kind", C.c_int), ("alpha", C.c_float), ("th_grad", C.c_float), ("reserved", C.c_int * 4)]
+                ("energy_kind", C.c_int), ("alpha", C.c_float), ("th_grad", C.c_float), ("filter", C.c_int),
+                ("reserved", C.c_int * 3)]
+
+
+FILTER_GF, FILTER_BILATERAL, FILTER_NONE = 0, 1, 2   # LEXP_FILTER_* of include/lexp_cuda.h
 
 
 class EvalResult(C.Structure):  # lexp_eval_result

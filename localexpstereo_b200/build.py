@@ -8,8 +8,12 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, "liblexp_cuda.so")
+# the kernels of the bilateral filter and the unfiltered mode (csrc/lexp_filters.cu) are a library of their own that liblexp_cuda.so
+# links (found next to it through its run path): liblexp_cuda.so keeps exactly the kernels it had before them
+FILTERS_SO = os.path.join(HERE, "liblexp_filters.so")
 SRCS = [os.path.join(HERE, "csrc", "lexp_capi.cu")]
-DEPS = SRCS + sorted(glob.glob(os.path.join(HERE, "csrc", "*.cuh"))) + [os.path.join(HERE, "..", "include", "lexp_cuda.h")]
+FILTERS_SRCS = [os.path.join(HERE, "csrc", "lexp_filters.cu")]
+DEPS = SRCS + FILTERS_SRCS + sorted(glob.glob(os.path.join(HERE, "csrc", "*.cuh"))) + [os.path.join(HERE, "..", "include", "lexp_cuda.h")]
 
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
@@ -18,9 +22,9 @@ NVCC_FLAGS = [
 
 
 def needs_build():
-    if not os.path.exists(SO):
+    if not os.path.exists(SO) or not os.path.exists(FILTERS_SO):
         return True
-    t = os.path.getmtime(SO)
+    t = min(os.path.getmtime(SO), os.path.getmtime(FILTERS_SO))
     return any(os.path.getmtime(d) > t for d in DEPS)
 
 
@@ -28,14 +32,17 @@ def build(force=False, verbose=False):
     if not force and not needs_build():
         return SO
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + ["-o", SO] + SRCS
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if verbose or res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-    if res.returncode != 0:
-        raise RuntimeError("nvcc failed building liblexp_cuda.so")
+    log = ""
+    for out, cmd in ((FILTERS_SO, [nvcc] + NVCC_FLAGS + ["-o", FILTERS_SO] + FILTERS_SRCS),
+                     (SO, [nvcc] + NVCC_FLAGS + ["-o", SO] + SRCS + ["-L", HERE, "-llexp_filters", "-Xlinker", "-rpath,$ORIGIN"])):
+        res = subprocess.run(cmd, capture_output=True, text=True)
+        if verbose or res.returncode != 0:
+            sys.stderr.write(res.stdout + res.stderr)
+        if res.returncode != 0:
+            raise RuntimeError(f"nvcc failed building {os.path.basename(out)}")
+        log += res.stdout + res.stderr
     with open(os.path.join(HERE, "build_ptxas.log"), "w") as f:
-        f.write(res.stdout + res.stderr)
+        f.write(log)
     return SO
 
 

@@ -8,6 +8,10 @@
 #include "lexp_ransac.cuh"
 #include "lexp_label_cost.cuh"
 #include "lexp_run.cuh"
+#include "lexp_filters.cuh"
+#ifdef LEXP_EMU
+#include "lexp_filters.cu"   // the emulator is one translation unit; the product links liblexp_filters.so
+#endif
 
 #include <algorithm>
 #include <cstdio>
@@ -165,6 +169,8 @@ struct lexp_ctx {
     size_t window_max = 0;
     bool smem_configured[3] = {false, false, false};   // [PM], [2]: the lean build of the PatchMatch-phase kernel
     bool lc_smem_configured[2] = {false, false};   // lexp_label_cost_kernel<NAIVE>: dynamic shared memory opt-in done
+    bool ft_smem_configured[2][2] = {};            // lexp_filter_unary_kernel<NAIVE, bilateral / none>: the same
+    float* d_bl_wtab = nullptr;                    // LEXP_FILTER_BILATERAL: exp(-s / sig2) for s = 0 .. 765 (lexp_filters.cuh)
     bool own_stream = true;
     bool vol_finite[2] = {false, false};
     // single-cell plans of lexp_eval_cell, keyed by (filterRect, targetRect): the unchanged reference loop calls the
@@ -248,6 +254,12 @@ cudaError_t launch_aux_smem(lexp_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3
 template <class... KArgs, class... Args>
 cudaError_t launch_aux(lexp_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, Args... args) {
     return launch_aux_smem(c, kern, grid, block, 0, args...);
+}
+// the launchers of lexp_filters.cu issue ordinary launches on the context's stream: the same bookkeeping as launch_aux
+cudaError_t launched_filter(lexp_ctx* c, cudaError_t e) {
+    c->chain_ok = false;
+    c->launches++;
+    return e;
 }
 
 int require_pm_state(const lexp_ctx* c, int mode) {
@@ -425,6 +437,36 @@ int check_rects(const lexp_ctx* c, const lexp_rect& f, const lexp_rect& t) {
     return LEXP_OK;
 }
 
+// the samplers' inputs of view `mode` (lexp_label_cost.cuh); the caller has checked that the view's inputs are set
+LcParams lc_params(const lexp_ctx* c, int mode) {
+    const int W = c->p.width;
+    LcParams lp{};
+    lp.vol = c->d_vol[mode]; lp.Wb = (W + 3) / 4;
+    lp.guide = c->d_guide[mode]; lp.statA = c->d_statA[mode]; lp.statB = c->d_statB[mode]; lp.statC = c->d_statC[mode];
+    lp.exi_own = c->d_exi[mode]; lp.exi_other = c->d_exi[1 - mode];
+    lp.label = c->d_cur_label[mode]; lp.cost = c->d_cur_cost[mode];
+    lp.H = c->p.height; lp.W = W; lp.D = c->p.ndisp; lp.R = c->R; lp.windR = c->p.windR; lp.mode = mode;
+    lp.th_col = c->p.th_col; lp.min_disp = c->p.min_disp; lp.max_disp = c->p.max_disp;
+    lp.thresh_color = c->p.th_col * (1.0f - c->p.alpha);    // StereoEnergy.h:663
+    lp.thresh_gradient = c->p.th_grad * c->p.alpha;          // StereoEnergy.h:664
+    return lp;
+}
+
+// The unary calls of a plan with the bilateral filter or none (lexp_filters.cuh): one ordinary launch, same outputs as the fused
+// kernel's: image with row pitch, or compact per-call tiles
+int launch_filter_unary(lexp_ctx* c, lexp_plan* pl, int mode, const Plane4* d_planes, float* d_out, long long pitch, int compact, int with_check) {
+    const bool naive = c->p.energy_kind == 1, bl = c->p.filter == LEXP_FILTER_BILATERAL;
+    const size_t smem = filter_unary_smem_bytes(c->p.windR, bl);
+    if (smem > c->smem_limit) return fail(LEXP_ERR_INVALID, "the filter kernel needs more shared memory than the device offers");
+    FtParams fp{};
+    fp.lc = lc_params(c, mode);
+    fp.items = pl->d_items; fp.planes = d_planes;
+    fp.out = d_out; fp.out_pitch = pitch; fp.out_compact = compact; fp.with_check = with_check;
+    fp.wtab = c->d_bl_wtab;
+    LEXP_CUDA(launched_filter(c, filter_launch_unary(naive, bl, fp, (unsigned)pl->nitems, smem, c->smem_limit, c->ft_smem_configured[naive][bl], c->stream)));
+    return LEXP_OK;
+}
+
 struct PmArgs {   // PatchMatch phase (lexp_plan_pm_step); nullptr = plain unary evaluation
     int pm_mode, prop_kind, prop_m, step_index;
     unsigned long long seed;
@@ -444,6 +486,10 @@ int run_plan(lexp_ctx* c, lexp_plan* pl, int mode, const Plane4* d_planes, float
     if (c->p.energy_kind == 1) {
         if (!c->d_exi[0] || !c->d_exi[1]) return fail(LEXP_ERR_STATE, "NaiveStereoEnergy needs the images of both views");
     } else if (!c->d_guide[mode] || !c->d_vol[mode]) return fail(LEXP_ERR_STATE, "image / volume of this view not set");
+    if (c->p.filter != LEXP_FILTER_GF) {   // the bilateral filter or none: lexp_filters.cuh (PatchMatch steps take the decomposed form)
+        if (pm) return fail(LEXP_ERR_INVALID, "internal: fused PatchMatch launch on a context without the guided filter");
+        return launch_filter_unary(c, pl, mode, d_planes, d_out, pitch, compact, with_check);
+    }
     if (c->persist_bytes && c->persist_mode != mode) {
         // keep the plane-independent inputs (statistics, guide) resident in L2 across the K steps of a group;
         // (the cost-volume gathers are plain read-only loads)
@@ -636,6 +682,9 @@ int lexp_create(const lexp_params* params, lexp_ctx** out_ctx) {
     if ((size_t)params->height * params->width >= (1ull << 30)) return fail(LEXP_ERR_INVALID, "image too large (H*W must be < 2^30)");
     if (params->windR < 2 || params->windR / 2 > 24) return fail(LEXP_ERR_INVALID, "windR/2 must be in [1, 24]");
     if (params->energy_kind != 0 && params->energy_kind != 1) return fail(LEXP_ERR_INVALID, "energy_kind must be 0 or 1");
+    if (params->filter < LEXP_FILTER_GF || params->filter > LEXP_FILTER_NONE) return fail(LEXP_ERR_INVALID, "filter must be one of LEXP_FILTER_*");
+    if (params->filter == LEXP_FILTER_BILATERAL && !(params->eps > 0.0f && std::isfinite(params->eps)))
+        return fail(LEXP_ERR_INVALID, "the bilateral filter needs sig2 (eps) > 0 and finite");
     int ndev = 0;
     LEXP_CUDA(cudaGetDeviceCount(&ndev));
     if (params->device < 0 || params->device >= ndev) return fail(LEXP_ERR_INVALID, "bad device ordinal");
@@ -681,6 +730,15 @@ int lexp_create(const lexp_params* params, lexp_ctx** out_ctx) {
     }
     if (max_tile_ow(c->R) < 8) { delete c; return fail(LEXP_ERR_INVALID, "windR too large for the tile width"); }
     LEXP_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+    if (c->p.filter == LEXP_FILTER_BILATERAL) {
+        // the weights of BilateralFilter::filter (GuidedFilter.h:362-363) for every channel sum: FP64, rounded once to float
+        float wtab[kBlWeights];
+        for (int s = 0; s < kBlWeights; s++) wtab[s] = (float)std::exp(-(double)s / (double)c->p.eps);
+        cudaError_t e = cudaMalloc(&c->d_bl_wtab, sizeof(wtab));
+        if (e == cudaSuccess) e = h2d(c, c->d_bl_wtab, wtab, sizeof(wtab));
+        if (e == cudaSuccess) e = cudaStreamSynchronize(c->stream);
+        if (e != cudaSuccess) { lexp_destroy(c); return fail(LEXP_ERR_CUDA, std::string("bilateral weights: ") + cudaGetErrorString(e)); }
+    }
     *out_ctx = c;
     return LEXP_OK;
 }
@@ -720,6 +778,7 @@ int lexp_destroy(lexp_ctx* c) {
     cudaFree(c->d_ransac_disp);
     cudaFree(c->d_gt);
     cudaFree(c->d_nonocc);
+    cudaFree(c->d_bl_wtab);
     if (c->h_gc_flags) cudaFreeHost(c->h_gc_flags);
     cudaFree(c->d_sync_arena);
     if (c->own_stream) cudaStreamDestroy(c->stream);
@@ -1346,6 +1405,10 @@ int lexp_pm_device_state(lexp_ctx* c, int mode, float** d_cost, lexp_plane** d_l
     return LEXP_OK;
 }
 
+namespace {
+int ensure_gc_plan_state(lexp_ctx* c, lexp_plan* pl, int mode);
+}  // namespace
+
 int lexp_plan_set_units(lexp_plan* pl, const lexp_rect* units, const int* cell_ids) {
     if (!pl || !units) return fail(LEXP_ERR_INVALID, "bad argument");
     lexp_ctx* c = pl->ctx;
@@ -1376,6 +1439,10 @@ int lexp_plan_set_units(lexp_plan* pl, const lexp_rect* units, const int* cell_i
         pl->sync_off = (long long)c->sync_used;
         c->sync_used += need;
     }
+    // the decomposed PatchMatch step of the bilateral filter / no filter (filter_pm_step) needs the proposal-cost images and the plan's
+    // cells: made here, so that its steps issue only graph-capturable work, as the fused steps do
+    if (c->p.filter != LEXP_FILTER_GF)
+        for (int m = 0; m < 2; m++) { int rc = ensure_gc_plan_state(c, pl, m); if (rc) return rc; }
     return LEXP_OK;
 }
 
@@ -1387,6 +1454,11 @@ int lexp_pm_reset_sync(lexp_ctx* c) {
     if (c->sync_used) LEXP_CUDA(memset0(c, c->d_sync_arena, c->sync_used));
     return LEXP_OK;
 }
+
+namespace {
+int filter_pm_step(lexp_ctx* c, lexp_plan* pl, int mode, int kind, int m, uint64_t seed, const lexp_plane* planes, int planes_on_device,
+                   lexp_plane* d_planes_out, int flags, int publish_epoch);
+}  // namespace
 
 int lexp_plan_pm_step_ex(lexp_ctx* c, lexp_plan* pl, int mode, int step_index, int kind, int m, uint64_t seed, const lexp_plane* planes,
                          int planes_on_device, lexp_plane* d_planes_out, int flags, int publish_epoch, const int* wait_epochs, unsigned wait_mask) {
@@ -1400,6 +1472,7 @@ int lexp_plan_pm_step_ex(lexp_ctx* c, lexp_plan* pl, int mode, int step_index, i
         return fail(LEXP_ERR_INVALID, "the image-based energy's PatchMatch phase runs on one GPU: this view is connected to peers");
     if (publish_epoch < 0 || (wait_mask >> kMaxPeers) || (wait_mask && !wait_epochs)) return fail(LEXP_ERR_INVALID, "bad epoch / mask");
     LEXP_ENTER(c);
+    if (c->p.filter != LEXP_FILTER_GF) return filter_pm_step(c, pl, mode, kind, m, seed, planes, planes_on_device, d_planes_out, flags, publish_epoch);
     const Plane4* dp = nullptr;   // the other kinds: the device proposers generate the planes
     if (kind == LEXP_PROP_LIST) {
         int rc = stage_planes(c, pl, planes, planes_on_device, &dp);
@@ -1463,6 +1536,36 @@ int ensure_gc_plan_state(lexp_ctx* c, lexp_plan* pl, int mode) {
     int rc = upload_gc_cells(c, pl->ncalls, pl->targ.data(), &pl->d_gc_cells, &pl->gc_nodes);
     if (rc) return rc;
     for (const lexp_rect& t : pl->targ) pl->gc_max_nodes = std::max(pl->gc_max_nodes, t.width * t.height);
+    return LEXP_OK;
+}
+
+// lexp_plan_pm_step[_ex] on a context with the bilateral filter or none: the fused kernel's step in its decomposed form -- the proposals
+// (the caller's list, the RANSAC fit, or lexp_gc_propose_kernel: the fused prologue's draws for the same state and launch seed), their
+// unary costs into the proposalCost image (run_plan), then lexp_filter_pm_update_kernel over the targetRects.  Ordinary stream-ordered
+// launches: every one starts after the previous ones have completed, so the fused path's per-cell counters are not needed; the group's
+// epoch flag is published as the fused path publishes it.  lexp_plan_set_units has made the plan's cells and the proposal-cost images.
+int filter_pm_step(lexp_ctx* c, lexp_plan* pl, int mode, int kind, int m, uint64_t seed, const lexp_plane* planes, int planes_on_device,
+                   lexp_plane* d_planes_out, int flags, int publish_epoch) {
+    { int rc = ensure_gc_plan_state(c, pl, mode); if (rc) return rc; }
+    const int W = c->p.width;
+    Plane4* dp = pl->d_planes;
+    if (kind == LEXP_PROP_LIST) {
+        const Plane4* staged = nullptr;
+        int rc = stage_planes(c, pl, planes, planes_on_device, &staged);
+        if (rc) return rc;
+        dp = const_cast<Plane4*>(staged);
+    } else if (kind == LEXP_PROP_RANSAC) {   // then read like a list
+        int rc = launch_ransac(c, pl, mode, seed);
+        if (rc) return rc;
+        kind = LEXP_PROP_LIST;
+    }
+    if (kind != LEXP_PROP_LIST || d_planes_out)
+        LEXP_CUDA(launch_aux(c, lexp_gc_propose_kernel, (pl->ncalls + 127) / 128, 128, pl->d_calls, pl->ncalls, dp, reinterpret_cast<Plane4*>(d_planes_out),
+                             (unsigned long long)seed, c->d_cur_label[mode], W, kind, m, c->p.min_disp, c->p.max_disp));
+    { int rc = run_plan(c, pl, mode, dp, c->d_prop_cost[mode], W, 0, 1); if (rc) return rc; }   // ComputeUnaryPotential (FastGCStereo.h:49)
+    LEXP_CUDA(launched_filter(c, filter_launch_pm_update((unsigned)pl->ncalls, pl->d_gc_cells, dp, c->d_prop_cost[mode], c->d_cur_cost[mode],
+                                                         c->d_cur_label[mode], W, (flags & LEXP_PM_INIT) ? 1 : 0, c->d_flags[mode],
+                                                         c->d_flags[mode] + kMaxPeers, c->peers[mode].rank, publish_epoch, c->stream)));
     return LEXP_OK;
 }
 
@@ -1638,6 +1741,11 @@ int lexp_pm_init_from_labeling(lexp_ctx* c, int mode) {
     lp.th_col = c->p.th_col; lp.min_disp = c->p.min_disp; lp.max_disp = c->p.max_disp;
     lp.thresh_color = c->p.th_col * (1.0f - c->p.alpha);    // StereoEnergy.h:663
     lp.thresh_gradient = c->p.th_grad * c->p.alpha;          // StereoEnergy.h:664
+    if (c->p.filter != LEXP_FILTER_GF) {   // the bilateral filter or none (lexp_filters.cuh)
+        const bool bl = c->p.filter == LEXP_FILTER_BILATERAL;
+        LEXP_CUDA(launched_filter(c, filter_launch_label_cost(naive, bl, lp, c->d_bl_wtab, c->stream)));
+        return LEXP_OK;
+    }
     auto kern = naive ? lexp_label_cost_kernel<true> : lexp_label_cost_kernel<false>;
     if (!c->lc_smem_configured[naive]) {
         LEXP_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)c->smem_limit));
@@ -1804,6 +1912,7 @@ int lexp_pm_ipc_export(lexp_ctx* c, int mode, void* out) {
 
 int lexp_pm_ipc_connect(lexp_ctx* c, int mode, int rank, int world, const void* all) {
     if (!c || !all || mode < 0 || mode > 1 || world < 1 || world > kMaxPeers || rank < 0 || rank >= world) return fail(LEXP_ERR_INVALID, "bad argument");
+    if (c->p.filter != LEXP_FILTER_GF) return fail(LEXP_ERR_INVALID, "the multi-GPU cell shard runs the guided filter only");
     { int rc = require_pm_state(c, mode); if (rc) return rc; }
 #ifdef LEXP_EMU
     return fail(LEXP_ERR_INVALID, "no inter-process memory on the emulator");
@@ -1832,6 +1941,7 @@ int lexp_pm_ipc_connect(lexp_ctx* c, int mode, int rank, int world, const void* 
 int lexp_pm_connect_local(lexp_ctx* c, int mode, int rank, int world, lexp_ctx* const* peer_ctx) {
     if (!c || !peer_ctx || mode < 0 || mode > 1 || world < 1 || world > kMaxPeers || rank < 0 || rank >= world) return fail(LEXP_ERR_INVALID, "bad argument");
     if (peer_ctx[rank] != c) return fail(LEXP_ERR_INVALID, "peer_contexts[rank] must be this context");
+    if (c->p.filter != LEXP_FILTER_GF) return fail(LEXP_ERR_INVALID, "the multi-GPU cell shard runs the guided filter only");
     LEXP_ENTER(c);
     lexp_ctx::Peers pr;
     int slot = 1;

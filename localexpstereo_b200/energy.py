@@ -249,15 +249,25 @@ class CostVolumeEnergy:
     """CostVolumeEnergy (CostVolumeEnergy.h:6-184) backed by the sm_90a kernels.
 
     imL / imR: uint8 [H][W][3] BGR; volL / volR: float32 [D][H][W] numpy arrays, or torch CUDA tensors /
-    integer device pointers (then no copy is made).  `params.filterName` must be "GF" or "GFfloat"
-    (both run the same FP32 kernel, within the 1e-4 tolerance of the reference's double filter)."""
+    integer device pointers (then no copy is made).  `params.filterName`, as the reference selects the filter
+    (CostVolumeEnergy.h:23-42): "GF" or "GFfloat" (both run the same FP32 guided-filter kernel, within the 1e-4 tolerance of the
+    reference's double filter), "BL" (bilateral filter, sig2 = filter_param1) or "" (no filter).  Any other name is rejected: the
+    reference leaves its filter a null pointer there and crashes on the first unary call."""
 
     ENERGY_KIND = 0
+    # filterName -> LEXP_FILTER_* (include/lexp_cuda.h)
+    FILTERS = {"GF": _capi.FILTER_GF, "GFfloat": _capi.FILTER_GF, "BL": _capi.FILTER_BILATERAL, "": _capi.FILTER_NONE}
+
+    @classmethod
+    def _filter_kind(cls, name):
+        if name not in cls.FILTERS:
+            raise LexpError(f'{cls.__name__} has no filter named "{name}": the reference leaves its filter a null pointer for that '
+                            f'name and crashes in ComputeUnaryPotential; use one of {sorted(cls.FILTERS)}')
+        return cls.FILTERS[name]
 
     def __init__(self, imL, imR, volL, volR, params: Parameters, MAX_DISPARITY, MIN_DISPARITY=0.0, MAX_VDISPARITY=0.0,
                  device: int = 0):
-        if params.filterName not in ("GF", "GFfloat"):
-            raise LexpError('only filterName "GF" / "GFfloat" is implemented on the GPU path')
+        filter_kind = self._filter_kind(params.filterName)
         if MAX_VDISPARITY != 0:
             raise LexpError("MAX_VDISPARITY != 0 is not supported (main.cpp never sets it)")
         imL = np.ascontiguousarray(imL, dtype=np.uint8)
@@ -267,7 +277,7 @@ class CostVolumeEnergy:
         D = self._ndisp(volL) if volL is not None else int(MAX_DISPARITY) + 1
         p = _capi.Params(self.height, self.width, D, int(params.windR), float(params.filter_param1), float(params.th_col),
                          float(MIN_DISPARITY), float(MAX_DISPARITY), int(device), int(self.ENERGY_KIND), float(params.alpha),
-                         float(params.th_grad))
+                         float(params.th_grad), filter_kind)
         h = C.c_void_p()
         check(lib().lexp_create(C.byref(p), C.byref(h)))
         self._h = h
@@ -548,8 +558,10 @@ class CostVolumeEnergy:
 class NaiveStereoEnergy(CostVolumeEnergy):
     """NaiveStereoEnergy (StereoEnergy.h:629-764): the image-based unary term of `-mode MiddV2` (BASELINE.json
     configs[0]) -- 4-channel ExI = [(1-alpha) BGR, alpha d/dx gray], other view warped with cv::warpAffine's fixed-point
-    bilinear sampling, truncated L1 colour + gradient cost, same guided-filter aggregation.  No cost volume."""
+    bilinear sampling, truncated L1 colour + gradient cost, aggregated as the reference selects (StereoEnergy.h:666-686): "GF" /
+    "GFfloat" (guided filter), "BF" (bilateral filter, sig2 = filter_param1) or "" (none).  No cost volume."""
     ENERGY_KIND = 1
+    FILTERS = {"GF": _capi.FILTER_GF, "GFfloat": _capi.FILTER_GF, "BF": _capi.FILTER_BILATERAL, "": _capi.FILTER_NONE}
 
     def __init__(self, imL, imR, params: Parameters, MAX_DISPARITY, MIN_DISPARITY=0.0, MAX_VDISPARITY=0.0, device: int = 0):
         if imL is None or imR is None:

@@ -37,6 +37,9 @@ def lib():
         L.oracle_unary.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int]
         L.oracle_unary_batch.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_int, C.c_int]
+        L.oracle_filter_unary_batch.restype = C.c_int
+        L.oracle_filter_unary_batch.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_int, C.c_int, C.c_int, C.c_double]
         L.oracle_max_threads.restype = C.c_int
         L.oracle_grid_mincut.argtypes = [C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_double)]
         _lib = L
@@ -48,6 +51,7 @@ class COracle:
         self.H, self.W, self.D = H, W, D
         self._h = lib().oracle_create(H, W, D, windR, eps, th_col, min_disp, max_disp)
         self._keep = {}
+        self._guide = set()
 
     def close(self):
         if self._h:
@@ -64,6 +68,7 @@ class COracle:
         bgr = np.ascontiguousarray(bgr, dtype=np.uint8)
         assert bgr.shape == (self.H, self.W, 3)
         lib().oracle_set_image(self._h, mode, bgr.ctypes.data)
+        self._guide.add(mode)
 
     def set_volume(self, mode, vol):
         vol = np.ascontiguousarray(vol, dtype=np.float32)
@@ -100,6 +105,30 @@ class COracle:
         lib().oracle_unary_batch(self._h, mode, len(fr), fr.ctypes.data, tr.ctypes.data, pl.ctypes.data,
                                  out_image.ctypes.data, int(with_check), int(nthreads))
         return out_image
+
+    FILTER_BILATERAL, FILTER_NONE = 1, 2   # LEXP_FILTER_BILATERAL, LEXP_FILTER_NONE
+
+    def filter_unary_batch(self, mode, frects, trects, planes, out_q=None, out_scale=None, with_check=True, filter=FILTER_BILATERAL,
+                           windR=None, sig2=10.0):
+        """The bilateral filter ("BL", radius windR, sig2 as the reference's float filter_param1) or none ("") of the cost-volume
+        energy on every call's targetRect: (q, sum w |p|) as float64 [H][W] images, written on the targetRects only."""
+        fr = np.ascontiguousarray(frects, dtype=np.int32).reshape(-1, 4)
+        tr = np.ascontiguousarray(trects, dtype=np.int32).reshape(-1, 4)
+        pl = np.ascontiguousarray(planes, dtype=np.float32).reshape(-1, 4)
+        assert len(fr) == len(tr) == len(pl) and mode in self._keep
+        if filter == self.FILTER_BILATERAL:
+            assert mode in self._guide and windR is not None
+        if out_q is None:
+            out_q = np.full((self.H, self.W), np.nan)
+        if out_scale is None:
+            out_scale = np.full((self.H, self.W), np.nan)
+        for a in (out_q, out_scale):
+            assert a.dtype == np.float64 and a.shape == (self.H, self.W) and a.flags.c_contiguous
+        if lib().oracle_filter_unary_batch(self._h, mode, len(fr), fr.ctypes.data, tr.ctypes.data, pl.ctypes.data, out_q.ctypes.data,
+                                           out_scale.ctypes.data, int(with_check), int(filter), int(windR or 0),
+                                           float(np.float32(sig2))):
+            raise ValueError(f"oracle_filter_unary_batch: filter {filter}, sig2 {sig2}")
+        return out_q, out_scale
 
 
 def max_threads():

@@ -288,6 +288,112 @@ void oracle_unary_batch(void* p, int mode, int ncalls, const int* frects, const 
     }
 }
 
+/* ------------------------------------------------------------------------------------------------------------------
+ * The reference's two other aggregation filters of CostVolumeEnergy (oracle/filter_oracle.py restates them in numpy):
+ *   filter 1, BilateralFilter::filter (GuidedFilter.h:329-373, filterName "BL"):
+ *       q(x) = sum over y in (x +- windR) & filterRect of p(y) exp(-(|B(y)-B(x)| + |G(y)-G(x)| + |R(y)-R(x)|) / sig2),
+ *     the 8-bit BGR guide of the view, the raw costs p of oracle_sample, not normalised;
+ *   filter 2, filterName "": the raw cost itself (CostVolumeEnergy.h:169-171).
+ * Weights exp(-s / sig2) in FP64 from a table over the integer channel sum s (0 .. 765: exact), window sums in FP64, the
+ * window walked row by row from the top and each row from the left (the numpy oracle's order).  out_q / out_scale are
+ * H x W double images: every call writes q and sum w |p| (|q| for "") on its targetRect; with_check sets both to
+ * COST_FOR_INVALID where IsValiLabel fails (CostVolumeEnergy.h:176-182).  One OpenMP thread per cell.
+ * ------------------------------------------------------------------------------------------------------------------ */
+#define ORACLE_FILTER_BILATERAL 1 /* LEXP_FILTER_BILATERAL */
+#define ORACLE_FILTER_NONE 2      /* LEXP_FILTER_NONE */
+
+/* StereoEnergy::IsValiLabel at (x, y) of targetRect (tw x th): the float arithmetic of oracle_unary_s's check */
+static int label_valid(const float* plane, int x, int y, int tw, int th, float MIN, float MAX) {
+    const float a = plane[0], b = plane[1], cc = plane[2], v = plane[3];
+    const float a5 = a * 5, b5 = b * 5;
+    float ds;
+    if (tw == 1 && th == 1) {
+        volatile float t0 = a * (float)x, t1 = b * (float)y;
+        volatile float t2 = t0 + t1;
+        ds = t2 + cc;
+    } else {
+        volatile float t0 = (float)x * a, t1 = (float)y * b, t2 = cc * 1.0f, t3 = 0.0f * v;
+        volatile float s = t0 + t1;
+        s = s + t2;
+        s = s + t3;
+        ds = s;
+    }
+    return valid_ds(ds, a5, b5, MIN, MAX);
+}
+
+typedef struct { size_t cap; float* raw; int* guide; } filter_scratch;
+
+static void oracle_filter_unary_s(oracle_ctx* c, int mode, const int* frect, const int* trect, const float* plane, double* out_q,
+                                  double* out_scale, int with_check, int filter, int R, const double* wtab, filter_scratch* sc) {
+    const int W = c->W;
+    const int fx = frect[0], fy = frect[1], fw = frect[2], fh = frect[3];
+    const int tx = trect[0], ty = trect[1], tw = trect[2], th = trect[3];
+    const size_t n = (size_t)fw * fh;
+    if (n > sc->cap) {
+        free(sc->raw); free(sc->guide);
+        sc->raw = (float*)malloc(n * sizeof(float));
+        sc->guide = (int*)malloc(n * 3 * sizeof(int));
+        sc->cap = n;
+    }
+    float* raw = sc->raw;
+    int* G = sc->guide;
+    oracle_sample(c, mode, fx, fy, fw, fh, plane, raw);
+    if (filter == ORACLE_FILTER_BILATERAL)   /* the 8-bit guide back from realI = B / 255 (exact after rounding) */
+        for (int y = 0; y < fh; y++)
+            for (int x = 0; x < fw; x++) {
+                const size_t i = (size_t)y * fw + x, g = (size_t)(fy + y) * W + fx + x;
+                for (int k = 0; k < 3; k++) G[i * 3 + k] = (int)lround(c->I[mode][k][g] * 255.0);
+            }
+    for (int y = ty; y < ty + th; y++)
+        for (int x = tx; x < tx + tw; x++) {
+            const size_t o = (size_t)y * W + x;
+            const size_t ci = (size_t)(y - fy) * fw + (x - fx);
+            double q, s;
+            if (filter == ORACLE_FILTER_BILATERAL) {
+                const int* g0 = G + ci * 3;
+                const int y0 = y - R < fy ? fy : y - R, y1 = y + R > fy + fh - 1 ? fy + fh - 1 : y + R;
+                const int x0 = x - R < fx ? fx : x - R, x1 = x + R > fx + fw - 1 ? fx + fw - 1 : x + R;
+                q = 0.0; s = 0.0;
+                for (int yy = y0; yy <= y1; yy++) {
+                    const size_t row = (size_t)(yy - fy) * fw - fx;
+                    for (int xx = x0; xx <= x1; xx++) {
+                        const int* g1 = G + (row + xx) * 3;
+                        const double w = wtab[abs(g1[0] - g0[0]) + abs(g1[1] - g0[1]) + abs(g1[2] - g0[2])];
+                        const double pv = (double)raw[row + xx];
+                        q += pv * w;
+                        s += fabs(pv) * w;
+                    }
+                }
+            } else {
+                q = (double)raw[ci];
+                s = fabs(q);
+            }
+            if (with_check && !label_valid(plane, x, y, tw, th, c->min_disp, c->max_disp)) q = s = (double)COST_FOR_INVALID;
+            out_q[o] = q;
+            out_scale[o] = s;
+        }
+}
+
+/* returns -1 for an unknown filter or a bilateral sig2 that is not positive */
+int oracle_filter_unary_batch(void* p, int mode, int ncalls, const int* frects, const int* trects, const float* planes, double* out_q,
+                              double* out_scale, int with_check, int filter, int windR, double sig2) {
+    oracle_ctx* c = (oracle_ctx*)p;
+    if (filter != ORACLE_FILTER_BILATERAL && filter != ORACLE_FILTER_NONE) return -1;
+    if (filter == ORACLE_FILTER_BILATERAL && !(sig2 > 0)) return -1;
+    double wtab[766];
+    for (int s = 0; s < 766; s++) wtab[s] = exp(-(double)s / sig2);
+#pragma omp parallel
+    {
+        filter_scratch sc = {0, NULL, NULL};
+#pragma omp for schedule(dynamic, 1)
+        for (int i = 0; i < ncalls; i++)
+            oracle_filter_unary_s(c, mode, frects + 4 * i, trects + 4 * i, planes + 4 * i, out_q, out_scale, with_check, filter, windR,
+                                  wtab, &sc);
+        free(sc.raw); free(sc.guide);
+    }
+    return 0;
+}
+
 int oracle_max_threads(void) {
 #ifdef _OPENMP
     return omp_get_max_threads();

@@ -129,10 +129,11 @@ def check_unary(dm, energy, filt, H, W, D, windR, mode=0, seed=0, MIN=0.0, MAX=N
         E.close()
 
 
-def check_warm_start(energy, filt, H, W, D, windR, mode=0, seed=0, MIN=0.0, MAX=None, unary_pixels=None):
-    """lexp_pm_init_from_labeling on independent random planes per pixel: every pixel against the oracle, and the pixels
-    `unary_pixels` (all: None) bit for bit against the unary call (F(p), {p}) of the same plane."""
-    E, Or = make(energy, filt, H, W, D, windR, seed, MIN, MAX)
+def check_warm_start(energy, filt, H, W, D, windR, mode=0, seed=0, MIN=0.0, MAX=None, unary_pixels=None, scene=None):
+    """lexp_pm_init_from_labeling on independent random planes per pixel: the pixels `unary_pixels` (a seeded sample; all: None)
+    against the oracle and bit for bit against the unary call (F(p), {p}) of the same plane.  scene: (imL, imR, volL, volR) in place
+    of make_scene's (the view `mode`'s image and volume are required)."""
+    E, Or = make(energy, filt, H, W, D, windR, seed, MIN, MAX, scene=scene)
     exact = filt == "none"
     try:
         lab = random_plane_field(H, W, E.MIN_DISPARITY, E.MAX_DISPARITY, 400 + seed, v=energy == "naive", nonfinite=0.02)

@@ -11,9 +11,13 @@ so it needs budgets.  Here every step starts from the device's own pre-step stat
   (U) update: nothing outside the group's targetRects changes; inside, post = (pre_cost > q) ? (q, plane) : pre bit for bit (a NaN
       cost never updates), or (q, plane) unconditionally for an initialisation.  q is the PatchMatch instantiation's own proposal
       cost: the recorded planes run as an initialisation on a twin context (same inputs, its own state and schedule);
-  (Q) q against an oracle of the energy: 1e-4 relative and the exact COST_FOR_INVALID mask.  Cost-volume energy: the FP64 C oracle
-      (oracle.c_oracle, which tests/test_ref_pin.py pins to the reference) on every target pixel, and the NaN pattern.  Image-based
-      energy: the numpy oracle on q_cells cells of every step, drawn from the rig's own random stream;
+  (Q) q against an oracle of the energy, with the exact COST_FOR_INVALID mask.  Guided filter ("GF"): 1e-4 relative; cost-volume
+      energy: the FP64 C oracle (oracle.c_oracle, which tests/test_ref_pin.py pins to the reference) on every target pixel, and the
+      NaN pattern; image-based energy: the numpy oracle on q_cells cells of every step, drawn from the rig's own random stream.
+      The bilateral filter ("BL" / "BF") and none (""), under the rules of tests/filter_checks.compare (NaN pattern exact, "" bit for
+      bit, bilateral |d| <= 1e-5 max(sum w |p|, 1e-3)): cost-volume energy on every target pixel against
+      COracle.filter_unary_batch (which tests/test_filter_c_oracle.py pins to oracle/filter_oracle.py), image-based energy on q_cells
+      cells against oracle/filter_oracle.py;
   (I) q equals the unary instantiation's cost of the same planes (Plan.eval_device: image output, with the check) bit for bit --
       the graph-cut steps take their proposal costs from that instantiation.
 run_sweep issues the steps one at a time with a synchronisation in between; the final state must equal the twin's uninterrupted sweep
@@ -21,14 +25,19 @@ bit for bit (tests/test_gpu_launch_chains.py shows that overlapped launches equa
 
 Pixel tags (cost-volume energy only): the fourth plane component v enters that cost only as 0 * v and through isfinite, and
 RandomProposer copies it.  With v = y * W + x in every pixel after the initialisation, a proposal names the pixel it was drawn from.
-In the image-based energy v shifts the warp, so it changes the cost: tagging that state raises."""
+The same holds with the bilateral filter and none ("BL" / ""), whose weights come from the guide alone.  In the image-based energy v
+shifts the warp, so it changes the cost: tagging that state raises."""
 import time
 
 import numpy as np
 
 from oracle import c_oracle
 from oracle import lexp_oracle as O
+import filter_checks as FC
 from lexp_testlib import assert_costs_close, bits
+
+NAIVE_FILTERS = ("GF", "BF", "")
+CV_FILTERS = ("GF", "BL", "")
 
 
 def ulps(a, b):
@@ -55,26 +64,36 @@ class Rig:
     """The context under test E and its twin Eq on the same inputs, a PMSweep on each, the oracle of the energy for (Q) and
     page-locked buffers for the states.  naive=False: CostVolumeEnergy on (imL, imR, volL, volR) (vol_host: a host copy of the view's
     volume for the C oracle, when that volume is on the device); naive=True: NaiveStereoEnergy on (imL, imR) with the parameters of
-    `-mode MiddV2` (volL, volR unused, MAX required), (Q) on q_cells cells per step drawn with np.random.default_rng(seed)."""
+    `-mode MiddV2` (volL, volR unused, MAX required), (Q) on q_cells cells per step drawn with np.random.default_rng(seed).
+    filter: the contexts' filterName -- "GF" (the guided filter, eps 1e-4), "BL" (cost volume) / "BF" (image-based): the bilateral
+    filter with sig2, "": none."""
 
     def __init__(self, devmem, imL, imR, volL, volR, windR, units, proposers, mode=0, MIN=0.0, MAX=None, vol_host=None, naive=False,
-                 q_cells=4, seed=0):
+                 q_cells=4, seed=0, filter="GF", sig2=10.0):
         import localexpstereo_b200 as L
         from localexpstereo_b200.sweep import PMSweep
         self.L, self.dm, self.mode, self.naive = L, devmem, mode, naive
         self.MIN = float(MIN)
+        assert filter in (NAIVE_FILTERS if naive else CV_FILTERS), f"filterName {filter!r}"
+        self.filter, self.windR, self.sig2 = filter, windR, sig2
         if naive:
-            from naive_pm_checks import middv2_params
-            prm = middv2_params(windR)
+            from naive_pm_checks import MIDDV2_LAMBDA, middv2_params
+            prm = middv2_params(windR) if filter == "GF" else L.Parameters(lambda_=MIDDV2_LAMBDA, windR=windR, filterName=filter,
+                                                                           filter_param1=sig2)
             self.MAX = float(MAX)
             self.E, self.Eq = [L.NaiveStereoEnergy(imL, imR, prm, self.MAX, self.MIN) for _ in range(2)]
-            self.Or = O.NaiveStereoEnergyOracle(imL, imR, windR, 1e-4, prm.th_col, prm.th_grad, prm.alpha, self.MAX, self.MIN)
+            if filter == "GF":
+                self.Or = O.NaiveStereoEnergyOracle(imL, imR, windR, 1e-4, prm.th_col, prm.th_grad, prm.alpha, self.MAX, self.MIN)
+            else:
+                from oracle.filter_oracle import FilteredEnergyOracle
+                self.Or = FilteredEnergyOracle.naive(imL, imR, windR, sig2, prm.th_col, prm.th_grad, prm.alpha, self.MAX, self.MIN,
+                                                     bilateral=filter == "BF")
             self.rng, self.q_cells = np.random.default_rng(seed), q_cells
         else:
             vol = volR if mode else volL
             D = int(vol.shape[0])
             self.MAX = float(D - 1 if MAX is None else MAX)
-            prm = L.Parameters(windR=windR, filterName="GF", filter_param1=1e-4, th_col=0.5)
+            prm = L.Parameters(windR=windR, filterName=filter, filter_param1=1e-4 if filter == "GF" else sig2, th_col=0.5)
             self.E, self.Eq = [L.CostVolumeEnergy(imL, imR, volL, volR, prm, self.MAX, self.MIN) for _ in range(2)]
         self.H, self.W = self.E.height, self.E.width
         self.S, self.Sq = [PMSweep(E, unit_sizes=units, proposers=proposers, mode=mode) for E in (self.E, self.Eq)]
@@ -88,6 +107,7 @@ class Rig:
             for a in self.buf[k]:
                 L.host_register(a)
         self.owner = {}
+        self.fq = None
         self.tags = (np.arange(self.H, dtype=np.float32)[:, None] * np.float32(self.W) + np.arange(self.W, dtype=np.float32)[None, :])
         self.tagged = self.tag_check_pending = False
         self.T = Tally()
@@ -201,12 +221,27 @@ class Rig:
             "(U) a pixel outside the step's targetRects changed"
         # (Q)
         t1 = time.perf_counter()
-        if self.naive:
+        if self.naive and self.filter != "GF":
+            for i in self.rng.choice(n, min(n, self.q_cells), replace=False):
+                x, y, w, h = targets[i]
+                ref, scale = self.Or.unary(filters[i], targets[i], used[i], self.mode)
+                T.worst_q = max(T.worst_q, FC.compare(q_c[y:y + h, x:x + w], ref, scale, self.filter == "",
+                                                      f"(Q) {self.filter!r} cell {ids[i]} plane {used[i]}"))
+                T.q_cells += 1
+        elif self.naive:
             for i in self.rng.choice(n, min(n, self.q_cells), replace=False):
                 x, y, w, h = targets[i]
                 ref = self.Or.compute_unary_potential(filters[i], targets[i], used[i], self.mode)
                 T.worst_q = max(T.worst_q, assert_costs_close(q_c[y:y + h, x:x + w], ref, f"(Q) cell {ids[i]} plane {used[i]}"))
                 T.q_cells += 1
+        elif self.filter != "GF":
+            if self.fq is None:
+                self.fq = (np.empty((self.H, self.W)), np.empty((self.H, self.W)))
+            fk = self.C.FILTER_NONE if self.filter == "" else self.C.FILTER_BILATERAL
+            ref, scale = self.C.filter_unary_batch(self.mode, filters, targets, used, *self.fq, with_check=True, filter=fk,
+                                                   windR=self.windR, sig2=self.sig2)
+            T.worst_q = max(T.worst_q, FC.compare(q, ref[inside], scale[inside], self.filter == "", f"(Q) {self.filter!r} step kind {kind} m {m}"))
+            T.q_cells += n
         else:
             ref = np.zeros((self.H, self.W), np.float32)
             self.C.unary_batch(self.mode, filters, targets, used, ref, with_check=True)
@@ -282,9 +317,10 @@ def assert_same_state(a, b, what):
     assert np.array_equal(bits(a[1]), bits(b[1])), f"{what}: currentLabeling differs"
 
 
-def run_sweep(R, labels, iterations, seed, what="scene"):
-    """The twin uninterrupted, then the sweep under test step by step with every step certified (the initialisation included);
-    the final states must be bit-identical.  The cost-volume energy's states are tagged after the initialisation."""
+def run_sweep(R, labels, iterations, seed, what="scene", layers=None):
+    """The twin uninterrupted, then the sweep under test step by step with every step certified (the initialisation included;
+    layers: only the steps of these layers, the others issued one by one uncertified); the final states must be bit-identical.
+    The cost-volume energy's states are tagged after the initialisation."""
     tag = not R.naive
     ref = R.twin_reference(labels, seed, (iterations - 1, len(R.S.unit_sizes) - 1), tag=tag)
     R.E.pm_begin(R.mode)
@@ -292,7 +328,7 @@ def run_sweep(R, labels, iterations, seed, what="scene"):
     if tag:
         R.tag(R.E)
     for it in range(iterations):
-        R.iteration(it, seed)
+        R.iteration(it, seed, certify=lambda g: layers is None or g.layer in layers)
     assert_same_state(R.get(R.E), ref, f"{what}: step by step against uninterrupted")
     print(R.T.line(what))
     return R.T

@@ -13,6 +13,7 @@
 #include "StereoEnergy.h"
 #endif
 #include <atomic>
+#include <cstdio>
 #include <cstring>
 #include <mutex>
 #include <stdexcept>
@@ -30,6 +31,7 @@ protected:
     float runPrecision_ = -1.0f, runThreshold_ = 0.5f;
     lexp_run_callback runCallback_ = nullptr;
     void* runUser_ = nullptr;
+    std::string saveDir_;                                            // setSaveDir: where run() writes the debug images
 
     static void check(int rc) {
         if (rc != LEXP_OK) throw std::runtime_error(std::string("lexp_cuda: ") + lexp_last_error());
@@ -143,6 +145,10 @@ public:
     // An empty `labeling` starts from random labels; a given H x W CV_32FC4 labeling is the start of every view.  On return `labeling` /
     // `rawlabeling` hold view 0 after / before the post-processing (H x W CV_32FC4).  setRunOptions: the run seed (the reference seeds
     // cv::theRNG() from the clock) and the Evaluator's precision / threshold with a callback at its points (lexp_set_ground_truth first).
+    // setSaveDir(dir): as `stereo.saveDir = outputDir + "debug\\"` with the Evaluator's saveDir (main.cpp:291-297): run() then writes the
+    // reference's debug images with cv::imwrite -- dir + "result{m}{D,N,E}{ii}.png" at every evaluation point and, with two views,
+    // dir + "result{0,1}C{ii}.png" after every iteration and the post-processing (lexp_run_ex, DESIGN.md 3j; needs lexp_set_ground_truth).
+    // An empty dir (the default) writes none.  setSaveDir exists where the cv:: layer has cv::imwrite and CV_8UC1 / CV_8UC3 (OpenCV does).
     void addLayer(int unitRegionSize, const std::vector<std::pair<int, int>>& proposers) {
         unitSizes_.push_back(unitRegionSize);
         layerProposers_.push_back(proposers);
@@ -151,6 +157,9 @@ public:
         runSeed_ = seed; runPrecision_ = precision; runThreshold_ = threshold; runCallback_ = callback; runUser_ = user;
     }
 #ifdef CV_32FC4   // OpenCV's Mat::create / CV_32FC4 (a cv:: stand-in without them leaves run out)
+#ifdef CV_8UC3    // and cv::imwrite of 8-bit images (a stand-in without CV_8UC3 leaves the debug images out)
+    void setSaveDir(const std::string& dir) { saveDir_ = dir; }
+#endif
     void run(int maxIteration, const std::vector<int>& viewModes, int pmInit, cv::Mat& labeling, cv::Mat& rawlabeling) const {
         const bool dual = viewModes.size() == 2 && viewModes[0] == 0 && viewModes[1] == 1;
         if (!dual && !(viewModes.size() == 1 && viewModes[0] == 0)) throw std::invalid_argument("run: viewModes must be {0} or {0, 1}");
@@ -165,7 +174,15 @@ public:
         std::vector<lexp_plane> lab((size_t)height_ * width_), raw((size_t)height_ * width_);
         lexp_run_options o{dual ? 2 : 1, pmInit, maxIteration, (int)unitSizes_.size(), unitSizes_.data(), np.data(), kind.data(), K.data(),
                            given ? reinterpret_cast<const lexp_plane*>(labeling.data) : nullptr, runSeed_, runPrecision_, runThreshold_};
-        check(lexp_run(ctx_, &o, lab.data(), raw.data(), runCallback_, runUser_));
+#ifdef CV_8UC3
+        if (!saveDir_.empty()) {
+            RunUser u{this, runUser_, false, std::string()};
+            const int rc = lexp_run_ex(ctx_, &o, lab.data(), raw.data(), runCallback_ ? forwardEvaluation : nullptr, writeImage, &u);
+            if (u.writeFailed) throw std::runtime_error("run: cv::imwrite failed for " + u.failedPath);
+            check(rc);
+        } else
+#endif
+            check(lexp_run(ctx_, &o, lab.data(), raw.data(), runCallback_, runUser_));
         labeling.create(height_, width_, CV_32FC4);
         rawlabeling.create(height_, width_, CV_32FC4);
         for (int y = 0; y < height_; y++) {
@@ -173,6 +190,29 @@ public:
             std::memcpy(rawlabeling.data + rawlabeling.step * (size_t)y, &raw[(size_t)y * width_], (size_t)width_ * sizeof(lexp_plane));
         }
     }
+
+#ifdef CV_8UC3
+private:
+    struct RunUser { const CudaCostVolumeEnergy* self; void* user; bool writeFailed; std::string failedPath; };
+    static void forwardEvaluation(void* u, int index, int mode, const lexp_eval_result* r, double seconds) {
+        const RunUser* ru = static_cast<const RunUser*>(u);
+        ru->self->runCallback_(ru->user, index, mode, r, seconds);
+    }
+    // Evaluator.h:164-166 (header "result") and FastGCStereo.h:164-165: one 8-bit image of lexp_run_ex, copied into a cv::Mat
+    static void writeImage(void* u, int index, int mode, int kind, const uint8_t* pixels, int width, int height, int channels) {
+        RunUser* ru = static_cast<RunUser*>(u);
+        if (ru->writeFailed) return;
+        cv::Mat m;
+        m.create(height, width, channels == 1 ? CV_8UC1 : CV_8UC3);
+        for (int y = 0; y < height; y++) std::memcpy(m.data + m.step * (size_t)y, pixels + (size_t)y * width * channels, (size_t)width * channels);
+        char name[64];
+        std::snprintf(name, sizeof name, "result%d%c%02d.png", mode, "DNEC"[kind], index);
+        const std::string path = ru->self->saveDir_ + name;
+        if (!cv::imwrite(path, m)) { ru->writeFailed = true; ru->failedPath = path; }
+    }
+
+public:
+#endif
 #endif
 
     lexp_ctx* context() const { return ctx_; }

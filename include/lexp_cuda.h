@@ -426,6 +426,32 @@ LEXP_API uint64_t lexp_run_seed(uint64_t run_seed, int mode, int phase, int iter
 LEXP_API int lexp_run(lexp_ctx* ctx, const lexp_run_options* options, lexp_plane* labeling_out, lexp_plane* raw_out,
                       lexp_run_callback callback, void* user);
 
+/* The reference's debug images (DESIGN.md 3j), rendered on the device.  8-bit, row-major; three-channel images are BGR interleaved. */
+/* Evaluator images of view `mode` (Evaluator.h:123-166): d = resultmD (the quantised disparity * 255 / max_disp), n_bgr = resultmN
+ * (computeNormalMap * 255), e = resultmE (255 correct or no GT, 200 wrong and occluded, 0 wrong), d, e [H][W], n_bgr [H][W][3]; any
+ * pointer may be NULL.  precision / threshold as lexp_evaluate.  Blocking, one read-back.
+ * LEXP_ERR_STATE without lexp_set_ground_truth or without the view's state. */
+LEXP_API int lexp_render_evaluation(lexp_ctx* ctx, int mode, float precision, float threshold, uint8_t* d, uint8_t* n_bgr, uint8_t* e);
+/* viewConsistencyCheck (PMStereoBase.h:87-108) of both views' current state: c0_bgr, c1_bgr [H][W][3] (either may be NULL): the
+ * disparity scaled by 255 / (max_disp - min_disp) from min_disp, blue where the other view's pixel is outside the image, red where the
+ * two disparities differ by more than 1.5.  Needs both views' state.  Blocking. */
+LEXP_API int lexp_render_consistency(lexp_ctx* ctx, uint8_t* c0_bgr, uint8_t* c1_bgr);
+#define LEXP_IMAGE_D 0
+#define LEXP_IMAGE_N 1
+#define LEXP_IMAGE_E 2
+#define LEXP_IMAGE_C 3
+/* One image of a run: `index` as lexp_run_callback's, `kind` one of LEXP_IMAGE_*, `channels` 1 (D, E) or 3 (N, C).  The pixels are
+ * valid only during the call. */
+typedef void (*lexp_run_image_callback)(void* user, int index, int mode, int kind, const uint8_t* pixels, int width, int height, int channels);
+/* lexp_run with the reference's debug images; lexp_run(...) == lexp_run_ex(..., NULL, user).  image_callback (nullable; needs
+ * lexp_set_ground_truth, else LEXP_ERR_STATE before anything is enqueued) receives D, N and E of lexp_render_evaluation(mode,
+ * options->precision, options->threshold) at every Evaluator point, after the evaluation callback; with two views also C of view 0 and
+ * of view 1 (lexp_render_consistency) after both views' evaluations of every pm and graph-cut iteration and after the post-processing
+ * (FastGCStereo.h:160-167,188-195,208-215).  The run's timer does not run while images are rendered and delivered, and the run computes
+ * the same labelings and evaluations with and without them. */
+LEXP_API int lexp_run_ex(lexp_ctx* ctx, const lexp_run_options* options, lexp_plane* labeling_out, lexp_plane* raw_out,
+                         lexp_run_callback callback, lexp_run_image_callback image_callback, void* user);
+
 /* LayerManager::addLayer (LayerManager.h:44-185): cell geometry of one layer.
  * Call with rect pointers == NULL to query counts.  group_of[r] = (i%4)*4 + (j%4) (LayerManager.h:168-173). */
 LEXP_API int lexp_layer_geometry(int width, int height, int windR, int unit_size, int* height_blocks,

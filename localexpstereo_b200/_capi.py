@@ -47,6 +47,9 @@ class RunOptions(C.Structure):  # lexp_run_options
 
 # lexp_run_callback(user, index, mode, result, seconds)
 RUN_CALLBACK = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.POINTER(EvalResult), C.c_double)
+# lexp_run_image_callback(user, index, mode, kind, pixels, width, height, channels)
+RUN_IMAGE_CALLBACK = C.CFUNCTYPE(None, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_uint8), C.c_int, C.c_int, C.c_int)
+IMAGE_KINDS = "DNEC"   # LEXP_IMAGE_D, _N, _E, _C of include/lexp_cuda.h
 
 # every symbol include/lexp_cuda.h declares: (restype, argtypes)
 _P = C.c_void_p
@@ -115,6 +118,9 @@ SYMBOLS = {
     "lexp_evaluate": (C.c_int, [_P, C.c_int, C.c_float, C.c_float, C.POINTER(EvalResult)]),
     "lexp_run_seed": (C.c_uint64, [C.c_uint64, C.c_int, C.c_int, C.c_int]),
     "lexp_run": (C.c_int, [_P, C.POINTER(RunOptions), _P, _P, RUN_CALLBACK, _P]),
+    "lexp_render_evaluation": (C.c_int, [_P, C.c_int, C.c_float, C.c_float, _P, _P, _P]),
+    "lexp_render_consistency": (C.c_int, [_P, _P, _P]),
+    "lexp_run_ex": (C.c_int, [_P, C.POINTER(RunOptions), _P, _P, RUN_CALLBACK, RUN_IMAGE_CALLBACK, _P]),
     "lexp_layer_geometry": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), _P, _P, _P, _P]),
 }
 

@@ -4,8 +4,11 @@ Arguments follow ArgsParser (ArgsParser.h): `-name value` pairs, booleans as tru
 the defaults, smooth_weight 1.0 for MiddV2 and 0.5 for MiddV3.  `-seed N` is an addition: the reference seeds cv::theRNG() from time(NULL)
 (main.cpp:430-450); here the run seed defaults to 0, so a command repeats its result.  `-threadNum` is accepted and ignored.
 
-Outputs as the reference's: disp0.pfm, disp0raw.pfm (-doDual only), time.txt and debug/log_output.txt (the Evaluator's log of view 0),
-and one console line per evaluation of view 0 (Evaluator.h:183).  The whole run is one lexp_run call on the device."""
+Outputs as the reference's: disp0.pfm, disp0raw.pfm (-doDual only), time.txt, debug/log_output.txt (the Evaluator's log of view 0),
+the Evaluator's images debug/result{m}D{ii}.png, result{m}N{ii}.png and result{m}E{ii}.png of every view at every evaluation
+(Evaluator.h:164-166), with -doDual the consistency-check images debug/result0C{ii}.png / result1C{ii}.png after every iteration and the
+post-processing (FastGCStereo.h:160-167,188-195,208-215), and one console line per evaluation of view 0 (Evaluator.h:183).  The whole
+run is one lexp_run_ex call on the device, which renders the images there."""
 from __future__ import annotations
 
 import os
@@ -79,6 +82,21 @@ def imread(path, gray=False):
         if gray:
             return np.array(im.convert("L"))
         return np.ascontiguousarray(np.array(im.convert("RGB"))[..., ::-1])
+
+
+def imwrite(path, image):
+    """cv::imwrite of an 8-bit image, gray [H][W] or BGR [H][W][3]: cv2 where it is importable, else PIL.  Raises if the file cannot be
+    written."""
+    try:
+        import cv2
+    except ImportError:
+        cv2 = None
+    if cv2 is not None:
+        if not cv2.imwrite(path, image):
+            raise OSError(f"could not write {path}")
+        return
+    from PIL import Image
+    Image.fromarray(np.ascontiguousarray(image[..., ::-1] if image.ndim == 3 else image)).save(path)
 
 
 def read_pfm(path):
@@ -219,8 +237,11 @@ def run(o, out=sys.stdout):
                 log.write("%f\t%f\t%f\t%f\t%f\t%f\n" % row)
                 log.flush()
                 out.write("%2d %5.1f\t%.0f\t%.0f\t%.0f\t%4.2f\t%4.2f\n" % ((index,) + row))
+            def image_cb(index, mode, kind, image):   # Evaluator.h:164-166 (header "result"), FastGCStereo.h:164-165
+                imwrite(os.path.join(outdir, "debug", "result%d%s%02d.png" % (mode, kind, index)), image)
             views = (0, 1) if o["doDual"] else (0,)
-            lab, raw = E.run(o["iterations"], views, o["pmIterations"], None, units, props, o["seed"], precision, threshold, callback=cb)
+            lab, raw = E.run(o["iterations"], views, o["pmIterations"], None, units, props, o["seed"], precision, threshold, callback=cb,
+                             image_callback=image_cb)
         from .energy import save_pfm_file
         save_pfm_file(os.path.join(outdir, "disp0.pfm"), disparities(lab))
         if o["doDual"]:

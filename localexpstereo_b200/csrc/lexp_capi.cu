@@ -9,8 +9,10 @@
 #include "lexp_label_cost.cuh"
 #include "lexp_run.cuh"
 #include "lexp_filters.cuh"
+#include "lexp_vis.cuh"
 #ifdef LEXP_EMU
 #include "lexp_filters.cu"   // the emulator is one translation unit; the product links liblexp_filters.so
+#include "lexp_vis.cu"       //                                                    and liblexp_vis.so
 #endif
 
 #include <algorithm>
@@ -145,6 +147,7 @@ struct lexp_ctx {
     int gc_big_nodes = 32768;                      // cells with more nodes run as phase kernels over all SMs (LEXP_GC_BIG_NODES)
     int* h_gc_flags = nullptr;                     // pinned: the two decision flags of the phase path
     char* d_post = nullptr;                        // lexp_post_process scratch: filled labelings, fail maps, row counts / offsets, list, weights
+    unsigned char* d_vis = nullptr;                // lexp_render_*: 8 bytes per pixel (D, N, E; or both fail maps and both C images)
     float* d_ransac_disp = nullptr;                // LEXP_PROP_RANSAC: float[H][W], the disparities of the snapshot of every cell's unitRegion
     float* d_gt = nullptr;                         // lexp_set_ground_truth: the left view's GT disparities float[H][W]
     unsigned char* d_nonocc = nullptr;             //                        and its non-occlusion mask (1: nonocc == 255)
@@ -255,7 +258,7 @@ template <class... KArgs, class... Args>
 cudaError_t launch_aux(lexp_ctx* c, void (*kern)(KArgs...), dim3 grid, dim3 block, Args... args) {
     return launch_aux_smem(c, kern, grid, block, 0, args...);
 }
-// the launchers of lexp_filters.cu issue ordinary launches on the context's stream: the same bookkeeping as launch_aux
+// the launchers of lexp_filters.cu and lexp_vis.cu issue ordinary launches on the context's stream: the same bookkeeping as launch_aux
 cudaError_t launched_filter(lexp_ctx* c, cudaError_t e) {
     c->chain_ok = false;
     c->launches++;
@@ -775,6 +778,7 @@ int lexp_destroy(lexp_ctx* c) {
     }
     cudaFree(c->d_gc_scratch);
     cudaFree(c->d_post);
+    cudaFree(c->d_vis);
     cudaFree(c->d_ransac_disp);
     cudaFree(c->d_gt);
     cudaFree(c->d_nonocc);
@@ -2240,18 +2244,73 @@ uint64_t lexp_run_seed(uint64_t run_seed, int mode, int phase, int iteration) { 
     return z ^ (z >> 31);
 }
 
+// The reference's debug images (lexp_vis.cuh): the kernels of liblexp_vis.so into the context's scratch d_vis, then a read-back of
+// the images the caller asks for, with one synchronisation
+static int ensure_vis(lexp_ctx* c) {
+    if (!c->d_vis) LEXP_CUDA(cudaMalloc(&c->d_vis, 8 * (size_t)c->p.height * c->p.width));
+    return LEXP_OK;
+}
+
+int lexp_render_evaluation(lexp_ctx* c, int mode, float precision, float threshold, uint8_t* d, uint8_t* n_bgr, uint8_t* e) {
+    if (!c || mode < 0 || mode > 1) return fail(LEXP_ERR_INVALID, "bad argument");
+    if (!c->d_gt) return fail(LEXP_ERR_STATE, "lexp_set_ground_truth has not been called");
+    { int rc = require_pm_state(c, mode); if (rc) return rc; }
+    LEXP_ENTER(c);
+    { int rc = ensure_vis(c); if (rc) return rc; }
+    const int H = c->p.height, W = c->p.width;
+    const size_t HW = (size_t)H * W;
+    unsigned char* dd = c->d_vis;            // D [H][W], N [H][W][3], E [H][W]
+    unsigned char* dn = c->d_vis + HW;
+    unsigned char* de = c->d_vis + 4 * HW;
+    LEXP_CUDA(launched_filter(c, vis_launch_eval(c->d_cur_label[mode], c->d_gt, c->d_nonocc, d ? dd : nullptr, n_bgr ? dn : nullptr, e ? de : nullptr, H, W,
+                                                 precision, threshold, c->p.max_disp, c->stream)));
+    if (d) LEXP_CUDA(d2h(c, d, dd, HW));
+    if (n_bgr) LEXP_CUDA(d2h(c, n_bgr, dn, 3 * HW));
+    if (e) LEXP_CUDA(d2h(c, e, de, HW));
+    LEXP_CUDA(cudaStreamSynchronize(c->stream));
+    return LEXP_OK;
+}
+
+int lexp_render_consistency(lexp_ctx* c, uint8_t* c0_bgr, uint8_t* c1_bgr) {
+    if (!c) return fail(LEXP_ERR_INVALID, "null ctx");
+    for (int m = 0; m < 2; m++) { int rc = require_pm_state(c, m); if (rc) return rc; }
+    LEXP_ENTER(c);
+    { int rc = ensure_vis(c); if (rc) return rc; }
+    const int H = c->p.height, W = c->p.width;
+    const size_t HW = (size_t)H * W;
+    unsigned char* d_fail = c->d_vis;        // fail [2][H][W] (doConsistencyCheck(.., 1.5), PMStereoBase.h:91), C [2][H][W][3]
+    unsigned char* d_c = c->d_vis + 2 * HW;
+    LEXP_CUDA(launch_aux(c, lexp_post_check_kernel, dim3((W + 127) / 128, H, 2), 128, c->d_cur_label[0], c->d_cur_label[1], d_fail, H, W, 1.5f));
+    LEXP_CUDA(launched_filter(c, vis_launch_check(c->d_cur_label[0], c->d_cur_label[1], d_fail, d_c, H, W, c->p.min_disp, c->p.max_disp, c->stream)));
+    if (c0_bgr) LEXP_CUDA(d2h(c, c0_bgr, d_c, 3 * HW));
+    if (c1_bgr) LEXP_CUDA(d2h(c, c1_bgr, d_c + 3 * HW, 3 * HW));
+    LEXP_CUDA(cudaStreamSynchronize(c->stream));
+    return LEXP_OK;
+}
+
 int lexp_run(lexp_ctx* c, const lexp_run_options* o, lexp_plane* labeling_out, lexp_plane* raw_out, lexp_run_callback callback, void* user) {
+    return lexp_run_ex(c, o, labeling_out, raw_out, callback, nullptr, user);
+}
+
+int lexp_run_ex(lexp_ctx* c, const lexp_run_options* o, lexp_plane* labeling_out, lexp_plane* raw_out, lexp_run_callback callback,
+                lexp_run_image_callback image_callback, void* user) {
     if (!c || !o || (o->n_views != 1 && o->n_views != 2) || o->pm_iterations < 0 || o->iterations < 0) return fail(LEXP_ERR_INVALID, "bad argument");
     if (callback && !c->d_gt) return fail(LEXP_ERR_STATE, "the callback evaluates the run: lexp_set_ground_truth first");
+    if (image_callback && !c->d_gt) return fail(LEXP_ERR_STATE, "the image callback renders the Evaluator's images: lexp_set_ground_truth first");
     if (o->n_views == 2 && !c->sm_set) return fail(LEXP_ERR_STATE, "lexp_set_smoothness has not been called: the post-processing needs omega");
     const int nv = o->n_views;
+    const int H = c->p.height, W = c->p.width;
+    const size_t HW = (size_t)H * W;
     std::vector<lexp_pm_sweep*> sw(nv, nullptr);
     auto done = [&](int rc) -> int { for (lexp_pm_sweep* s : sw) lexp_pm_sweep_destroy(s); return rc; };
     for (int m = 0; m < nv; m++) {
         int rc = lexp_pm_sweep_create(c, m, o->n_layers, o->unit_sizes, o->n_proposers, o->proposer_kind, o->proposer_K, 0, 1, &sw[m]);
         if (rc) return done(rc);
     }
-    // the Evaluator's timer (TimeStamper): runs from the end of the initialisation, stopped while evaluating
+    std::vector<uint8_t> img;   // host pixels handed to image_callback: D, N, E of one view, or C of both views
+    if (image_callback) img.resize(6 * HW);
+    // the Evaluator's timer (TimeStamper): runs from the end of the initialisation, stopped while evaluating and while the debug images
+    // are rendered and delivered (STOP_TIMER / START_TIMER, FastGCStereo.h:160-167)
     using clk = std::chrono::steady_clock;
     double elapsed = 0.0;
     clk::time_point t0;
@@ -2259,11 +2318,30 @@ int lexp_run(lexp_ctx* c, const lexp_run_options* o, lexp_plane* labeling_out, l
     auto evaluate = [&](int index, int mode) -> int {
         int rc = lexp_sync(c);
         if (ticking) elapsed += std::chrono::duration<double>(clk::now() - t0).count();
-        if (rc || !callback) { t0 = clk::now(); return rc; }
-        lexp_eval_result r{};
-        rc = lexp_evaluate(c, mode, o->precision, o->threshold, &r);
+        if (rc || (!callback && !image_callback)) { t0 = clk::now(); return rc; }
+        if (callback) {
+            lexp_eval_result r{};
+            rc = lexp_evaluate(c, mode, o->precision, o->threshold, &r);
+            if (rc) return rc;
+            callback(user, index, mode, &r, elapsed);
+        }
+        if (image_callback) {   // Evaluator.h:164-166
+            rc = lexp_render_evaluation(c, mode, o->precision, o->threshold, img.data(), img.data() + HW, img.data() + 4 * HW);
+            if (rc) return rc;
+            image_callback(user, index, mode, LEXP_IMAGE_D, img.data(), W, H, 1);
+            image_callback(user, index, mode, LEXP_IMAGE_N, img.data() + HW, W, H, 3);
+            image_callback(user, index, mode, LEXP_IMAGE_E, img.data() + 4 * HW, W, H, 1);
+        }
+        t0 = clk::now();
+        return LEXP_OK;
+    };
+    auto check_images = [&](int index) -> int {   // viewConsistencyCheck + imwrite of result0C / result1C (two views only)
+        if (!image_callback || nv != 2) return LEXP_OK;
+        int rc = lexp_sync(c);
+        if (ticking) elapsed += std::chrono::duration<double>(clk::now() - t0).count();
+        if (!rc) rc = lexp_render_consistency(c, img.data(), img.data() + 3 * HW);
         if (rc) return rc;
-        callback(user, index, mode, &r, elapsed);
+        for (int m = 0; m < 2; m++) image_callback(user, index, m, LEXP_IMAGE_C, img.data() + 3 * HW * m, W, H, 3);
         t0 = clk::now();
         return LEXP_OK;
     };
@@ -2275,22 +2353,29 @@ int lexp_run(lexp_ctx* c, const lexp_run_options* o, lexp_plane* labeling_out, l
     }
     t0 = clk::now();
     ticking = true;
-    for (int it = 0; it < o->pm_iterations; it++)   // :143-157
+    for (int it = 0; it < o->pm_iterations; it++) {   // :143-167
         for (int m = 0; m < nv; m++) {
             int rc = lexp_pm_sweep_iteration(sw[m], it, lexp_run_seed(o->seed, m, 1, it), nullptr);
             if (!rc) rc = evaluate(it + 1, m);
             if (rc) return done(rc);
         }
-    for (int it = 0; it < o->iterations; it++)      // :171-184
+        int rc = check_images(it + 1);
+        if (rc) return done(rc);
+    }
+    for (int it = 0; it < o->iterations; it++) {      // :171-195
         for (int m = 0; m < nv; m++) {
             int rc = lexp_pm_sweep_gc_iteration(sw[m], it, lexp_run_seed(o->seed, m, 2, it), nullptr);
             if (!rc) rc = evaluate(it + 1 + o->pm_iterations, m);
             if (rc) return done(rc);
         }
-    if (nv == 2) {   // rawlabeling = currentLabeling_[0].clone(); postProcess(.., 1.5) (:199-205)
+        int rc = check_images(it + 1 + o->pm_iterations);
+        if (rc) return done(rc);
+    }
+    if (nv == 2) {   // rawlabeling = currentLabeling_[0].clone(); postProcess(.., 1.5) (:199-215)
         int rc = raw_out ? lexp_pm_get(c, 0, nullptr, raw_out) : LEXP_OK;
         if (!rc) rc = lexp_post_process(c, 1.5f, nullptr);
         for (int m = 0; m < 2 && !rc; m++) rc = evaluate(o->iterations + 1 + o->pm_iterations, m);
+        if (!rc) rc = check_images(o->iterations + 1 + o->pm_iterations);
         if (!rc && labeling_out) rc = lexp_pm_get(c, 0, nullptr, labeling_out);
         return done(rc);
     }

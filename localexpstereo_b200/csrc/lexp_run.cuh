@@ -44,6 +44,21 @@ __device__ __forceinline__ int eval_cvround(double s) {
     return (s >= -2147483648.5 && s < 2147483647.5) ? __double2int_rn(s) : INT_MIN;
 }
 
+// The Evaluator's arithmetic at one pixel (Evaluator.h:123-139), shared by lexp_eval_kernel and the debug images of lexp_vis.cuh:
+// the disparity of `label` at (x, y), quantised when precision > 0 (returned in d), whether GT g is valid, and errorMap's predicate.
+__device__ __forceinline__ float eval_pixel(const float4 label, float g, int x, int y, float precision, float threshold, int& valid, int& ok) {
+    float d = gc_disp(label, (float)x, (float)y);
+    if (precision > 0.0f) {   // quantize (Evaluator.h:105-110): m.convertTo(CV_32S, 1.0 / precision), then back with scale precision
+        // cvtScale 32f -> 32s works in float: (float)src * (float)alpha + (float)beta, then cvRound; 32s -> 32f works in double
+        const float s = __fadd_rn(__fmul_rn(d, (float)__ddiv_rn(1.0, (double)precision)), 0.0f);
+        const int q = eval_cvround((double)s);
+        d = (float)__dmul_rn((double)q, (double)precision);
+    }
+    valid = (g > 0.0f && g <= 3.402823466e+38f) ? 1 : 0;   // validMask = GT > 0 & GT != inf
+    ok = ((double)fabsf(__fsub_rn(d, g)) <= (double)threshold) ? 1 : 0;   // errorMap = |disp - GT| <= errorThreshold
+    return d;
+}
+
 // part[4 b + k], k = valid pixels, nonocc pixels, correct & valid, correct & nonocc of block b
 __global__ void __launch_bounds__(kEvalThreads) lexp_eval_kernel(const float4* __restrict__ cur_label, const float* __restrict__ gt,
                                                                  const unsigned char* __restrict__ nonocc, long long* __restrict__ part, int H, int W,
@@ -53,17 +68,8 @@ __global__ void __launch_bounds__(kEvalThreads) lexp_eval_kernel(const float4* _
     int valid = 0, nocc = 0, ok = 0;
     if (p < (long long)H * W) {
         const int x = (int)(p % W), y = (int)(p / W);
-        float d = gc_disp(cur_label[p], (float)x, (float)y);
-        if (precision > 0.0f) {   // quantize (Evaluator.h:105-110): m.convertTo(CV_32S, 1.0 / precision), then back with scale precision
-            // cvtScale 32f -> 32s works in float: (float)src * (float)alpha + (float)beta, then cvRound; 32s -> 32f works in double
-            const float s = __fadd_rn(__fmul_rn(d, (float)__ddiv_rn(1.0, (double)precision)), 0.0f);
-            const int q = eval_cvround((double)s);
-            d = (float)__dmul_rn((double)q, (double)precision);
-        }
-        const float g = gt[p];
-        valid = (g > 0.0f && g <= 3.402823466e+38f) ? 1 : 0;   // validMask = GT > 0 & GT != inf
+        eval_pixel(cur_label[p], gt[p], x, y, precision, threshold, valid, ok);
         nocc = nonocc[p] ? 1 : 0;
-        ok = ((double)fabsf(__fsub_rn(d, g)) <= (double)threshold) ? 1 : 0;   // errorMap = |disp - GT| <= errorThreshold
     }
     s_bits[threadIdx.x] = (unsigned char)(valid | nocc << 1 | (ok & valid) << 2 | (ok & nocc) << 3);
     __syncthreads();

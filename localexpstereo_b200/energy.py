@@ -415,12 +415,33 @@ class CostVolumeEnergy:
         check(lib().lexp_evaluate(self._h, int(mode), float(precision), float(threshold), C.byref(r)))
         return self._eval_dict(r)
 
+    def render_evaluation(self, mode=0, precision=-1.0, threshold=0.5):
+        """The images Evaluator::evaluate writes for view `mode` (Evaluator.h:123-166, lexp_render_evaluation), rendered on the device:
+        (D, N, E) = the quantised disparity * 255 / MAX_DISPARITY as uint8 [H][W], the normal map as uint8 [H][W][3] (BGR) and the error
+        map as uint8 [H][W] (255 correct or no ground truth, 200 wrong and occluded, 0 wrong).  set_ground_truth first."""
+        H, W = self.height, self.width
+        d, n, e = np.empty((H, W), np.uint8), np.empty((H, W, 3), np.uint8), np.empty((H, W), np.uint8)
+        check(lib().lexp_render_evaluation(self._h, int(mode), float(precision), float(threshold), d.ctypes.data, n.ctypes.data, e.ctypes.data))
+        return d, n, e
+
+    def render_consistency(self):
+        """The images of PMStereoBase::viewConsistencyCheck (PMStereoBase.h:87-108, lexp_render_consistency) of both views' device state:
+        (C0, C1), uint8 [H][W][3] (BGR) each: the disparity in gray, blue where the other view's pixel is outside the image, red where
+        the two views' disparities differ by more than 1.5."""
+        H, W = self.height, self.width
+        c0, c1 = np.empty((H, W, 3), np.uint8), np.empty((H, W, 3), np.uint8)
+        check(lib().lexp_render_consistency(self._h, c0.ctypes.data, c1.ctypes.data))
+        return c0, c1
+
     def run(self, maxIteration, viewModes=(0, 1), pmInit=0, labeling=None, unit_sizes=None, proposers=None, seed=0, precision=-1.0,
-            threshold=0.5, callback=None):
-        """FastGCStereo::run(maxIteration, viewModes, pmInit, labeling, rawlabeling) on the device (lexp_run): random start (or the
+            threshold=0.5, callback=None, image_callback=None):
+        """FastGCStereo::run(maxIteration, viewModes, pmInit, labeling, rawlabeling) on the device (lexp_run_ex): random start (or the
         given Plane [H][W] labeling), pmInit PatchMatch iterations, maxIteration graph-cut iterations and, with viewModes (0, 1), the
         post-processing.  unit_sizes / proposers: the layers and their [(kind, K)] lists (default: sweep.v3_layer_units and
         sweep.V3_PROPOSERS_REFERENCE).  callback(index, mode, result_dict, seconds) at the Evaluator's points (set_ground_truth first).
+        image_callback(index, mode, kind, array) receives the reference's debug images (lexp_run_ex): kind "D", "N", "E" at every
+        Evaluator point after `callback`, and with two views "C" of view 0 and view 1 after every iteration and the post-processing;
+        the arrays are copies (uint8 [H][W] or [H][W][3] BGR).  Rendering does not count towards `seconds`.
         Returns (labeling, rawlabeling) of view 0, float32 [H][W][4] each."""
         from .sweep import V3_PROPOSERS_REFERENCE, v3_layer_units
         views = tuple(viewModes)
@@ -447,8 +468,16 @@ class CostVolumeEnergy:
                 callback(int(index), int(mode), self._eval_dict(res.contents), float(seconds))
             except BaseException as e:   # an exception cannot cross the C frames: re-raised after the run
                 errors.append(e)
+        def image_tramp(_user, index, mode, kind, pixels, width, height, channels):
+            try:
+                shape = (height, width) if channels == 1 else (height, width, channels)
+                a = np.ctypeslib.as_array(pixels, shape=shape).copy()
+                image_callback(int(index), int(mode), _capi.IMAGE_KINDS[kind], a)
+            except BaseException as e:
+                errors.append(e)
         cb = _capi.RUN_CALLBACK(tramp) if callback is not None else _capi.RUN_CALLBACK()
-        check(lib().lexp_run(self._h, C.byref(o), lab.ctypes.data, raw.ctypes.data, cb, None))
+        icb = _capi.RUN_IMAGE_CALLBACK(image_tramp) if image_callback is not None else _capi.RUN_IMAGE_CALLBACK()
+        check(lib().lexp_run_ex(self._h, C.byref(o), lab.ctypes.data, raw.ctypes.data, cb, icb, None))
         if errors:
             raise errors[0]
         return lab, raw

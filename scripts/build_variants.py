@@ -22,7 +22,7 @@ def main(names):
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     for name in names or VARIANTS:
         so = os.path.join(out_dir, f"liblexp_cuda_{name}.so")
-        r = subprocess.run([nvcc] + B.NVCC_FLAGS + VARIANTS[name] + ["-o", so] + B.SRCS + ["-L", B.HERE, "-llexp_filters", "-Xlinker", f"-rpath,{B.HERE}"], capture_output=True, text=True)
+        r = subprocess.run([nvcc] + B.NVCC_FLAGS + VARIANTS[name] + ["-o", so] + B.SRCS + ["-L", B.HERE, "-llexp_filters", "-llexp_vis", "-Xlinker", f"-rpath,{B.HERE}"], capture_output=True, text=True)
         if r.returncode:
             print(r.stderr[-3000:])
             raise SystemExit(f"variant {name} failed to build")
